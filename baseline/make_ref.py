@@ -26,7 +26,11 @@ DST = HERE / "_ref" / "ptwt"
 def make(force: bool = False) -> Path | None:
     if DST.exists() and not force:
         return DST
-    if not SRC.exists():
+    try:
+        present = SRC.is_dir()
+    except OSError:          # a reference checkout the building user may not read counts as absent
+        present = False
+    if not present:
         return None
     if DST.exists():
         shutil.rmtree(DST)

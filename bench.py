@@ -1,9 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- the BASELINE.json benchmarks of the B200 wavelet filter bank.
+"""bench.py -- the BASELINE.json benchmarks of the H100 wavelet filter bank.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5] [--gather]
+                    [--dump-outputs DIR]
 
 One "step" = one multi-level forward transform of one batch of synthetic data (per GPU).  Prints ONE JSON line (rank 0).
+--dump-outputs DIR writes the coefficients of the last timed step as DIR/coeffNN.npy (a fixed, seeded sample of each
+array when all of them exceed 64 MB), so that two builds can be compared output for output on identical inputs.
 
   --config 2  (default, the headline)  wavedec2  db4  level 4  reflect   64 x 4096 x 4096      float32
   --config 3                           wavedec3  sym4 level 3  zero       8 x 256 x 256 x 256  float32
@@ -16,6 +19,7 @@ See DESIGN.md section "Measurement" for every field.
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -93,11 +97,11 @@ def samples_of(shape) -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe).  The sampler is started
-    while the GPU is still idle (nvidia-smi needs a few hundred ms to come up, longer on an 8-GPU box; no load is added
-    before the timed region: a long pre-load pushes the part into its 1 kW power cap, 1965 -> ~1630 MHz) and the samples
-    are cut to the timed window by their timestamps; if the window is shorter than the sampling period, all samples since
-    the start are used and the record says so."""
+    """nvidia-smi clocks + throttle reasons during the timed region.  The sampler is started while the GPU is still idle
+    (nvidia-smi needs a few hundred ms to come up, longer on an 8-GPU machine; no load is added before the timed region: a
+    long pre-load can push the part into its power cap and lower the clock) and the samples are cut to the timed window
+    by their timestamps; if the window is shorter than the sampling period, all samples since the start are used and the
+    record says so."""
 
     Q = ("timestamp,index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -116,12 +120,17 @@ class ClockSampler:
                  "-i", str(self.index)], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             self.thread = threading.Thread(target=self._pump, daemon=True)
             self.thread.start()
+            atexit.register(self._kill)         # never leave the sampler running, whatever ends the benchmark
         except Exception:  # noqa: BLE001
             self.proc = None
 
     def _pump(self):
         for line in self.proc.stdout:
             self.lines.append((time.time(), line.strip()))
+
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.kill()
 
     def window_begin(self):
         self.t0 = time.time()
@@ -173,7 +182,7 @@ def measured_peak_gbs() -> tuple[float, str]:
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 # --------------------------------------------------------------------------------------------------------------
@@ -264,6 +273,27 @@ def describe(cfg, batch) -> str:
     return f"{name} {cfg['wavelet']} level={cfg['level']}{extra}, batch {batch} x {shp} {cfg['dtype']}"
 
 
+DUMP_BYTES = 60_000_000                       # under 64 MB with the .npy headers
+
+
+def dump_outputs(coeffs, out_dir: Path) -> None:
+    """The arrays a caller of the timed path receives, in their dtype (float32 / float64), as out_dir/coeffNN.npy in
+    the order of flat().  When they exceed 64 MB in all, each array is replaced by the same share of its elements at
+    fixed, seeded flat indices (drawn with replacement, sorted), so that two runs with the same arguments write comparable files."""
+    import numpy as np
+
+    ts = flat(coeffs)
+    total = nbytes(ts)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    g = torch.Generator().manual_seed(0)
+    for j, t in enumerate(ts):
+        if total > DUMP_BYTES:
+            k = max(1, t.numel() * DUMP_BYTES // total)
+            idx = torch.randint(t.numel(), (k,), generator=g).sort().values
+            t = t.reshape(-1)[idx.to(t.device)]
+        np.save(out_dir / f"coeff{j:02d}.npy", t.detach().cpu().numpy())
+
+
 # --------------------------------------------------------------------------------------------------------------
 # host placement: each rank on the NUMA node of its GPU, before the first pinned allocation
 # --------------------------------------------------------------------------------------------------------------
@@ -334,7 +364,11 @@ def main() -> None:
     ap.add_argument("--no-numa", action="store_true")
     ap.add_argument("--no-incumbent", action="store_true", help="skip timing the reference algorithm on the GPU")
     ap.add_argument("--incumbent-batch", type=int, default=16)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the coefficients of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     cfg = CONFIGS[args.config]
     if args.impl == "reference":
         run_reference(args, cfg)
@@ -421,6 +455,8 @@ def main() -> None:
     ms_per_step = total_ms / args.steps
     value = world * n_samples / (ms_per_step * 1e-3) / 1e6
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, Path(args.dump_outputs))
     _dbg("timed region done")
     # parity of what was just timed against the oracle, outside the timed region: items from BOTH halves of the batch
     # (the second half runs on the library's auxiliary stream with reused scratch slots in the 2-D analysis)
@@ -428,10 +464,7 @@ def main() -> None:
     if rank == 0:
         from oracle import ptwt_port as P
 
-        # matrix configuration: the port materialises the dense n x n operator before sparsifying it (34 GB at
-        # n = 65536); the unmodified reference builds the same operator sparsely (slow Python, little memory)
-        pmod = reference_module()[0] if cfg["kind"] == "matrix" else P
-        ofwd = make_forward(pmod, cfg)
+        ofwd = make_forward(P, cfg)
         items = sorted({0, B // 2 - 1, B // 2, B - 1} & set(range(B)))
         fg = flat(out)
         worst = 0.0
@@ -465,17 +498,6 @@ def main() -> None:
     k_launches = _native.launch_count()
     k_ms = k0.elapsed_time(k1) / 20
     achieved = alg_k / (k_ms * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    tf = ROOT / "profiles" / "traffic.json"
-    if tf.exists():
-        try:
-            tj = json.loads(tf.read_text())
-            traffic = tj.get(f"config{args.config}", {}).get("dominant_kernel_dram_bytes_per_launch")
-            if traffic is None and args.config == 2:
-                traffic = tj.get("dominant_kernel_dram_bytes_per_launch")
-            traffic_src = "static: one ncu --set full capture kept in profiles/traffic.json (not re-measured by this run)"
-        except Exception:  # noqa: BLE001
-            traffic = None
 
     _dbg("kernel timing done")
     # inverse transform of the same coefficients (reported separately, SURVEY.md section 8d)
@@ -572,7 +594,7 @@ def main() -> None:
             incumbent = {"value": samples_of(xs.shape) / (inc_ms * 1e-3) / 1e6, "unit": "Msamples/s (1 GPU)", "ms": inc_ms,
                          "sample": f"{nb} items, device resident",
                          "step_frac": alg * nb / B / (inc_ms * 1e-3) / 1e9 / peak,
-                         "what": "reference algorithm (F.pad + conv stride 2, torch/cuDNN) on the same B200"}
+                         "what": "reference algorithm (F.pad + conv stride 2, torch/cuDNN) on the same GPU"}
             del ref_c, xs
             torch.cuda.empty_cache()
         except Exception as ex:  # noqa: BLE001
@@ -590,12 +612,12 @@ def main() -> None:
             "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": cfg["dtype"], "data": "synthetic (torch.randn on device, seed 1234+rank)",
             "config": {"workload": f"{describe(cfg, B)} per GPU ({cfg['baseline_cfg']})",
-                       "l2": f"inputs ({in_mb:.0f} MB) and outputs ({out_mb:.0f} MB) exceed the 126 MB L2; no flush needed",
+                       "l2": f"inputs ({in_mb:.0f} MB) and outputs ({out_mb:.0f} MB) exceed the 50 MB L2; no flush needed",
                        "parallelism": f"batch-sharded x{world}, no data-path collective"
                                       + (" (+ all_gather of the results, reported under 'gather')" if gather else ""),
                        "numa": numa},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "kernel": cfg["kernel"],
                          "kernel_algorithmic_bytes_per_launch": alg_k, "kernel_ms_per_launch": k_ms,
                          "kernel_launches_timed": int(k_launches),

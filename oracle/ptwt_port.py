@@ -22,9 +22,8 @@ path instead of the reference's three per-dimension modules:
   matrix FWT             sameshift strided conv matrix, rows with nnz != L replaced by a dense QR
                          matmul_transform.py:47-165, 310-430, 603-703; sparse_math.py:253-311, 350-405, 482-516
 
-Parity is PINNED: tests/test_oracle_vs_reference.py compares every function here with the
-unmodified reference (imported from /root/reference when present) and with the committed golden
-fixtures under tests/golden/ that oracle/make_golden.py generated from the reference.
+Parity is PINNED: tests/test_oracle.py compares every function here with the committed golden fixtures
+under tests/golden/ that oracle/make_golden*.py generated from the unmodified reference.
 """
 from __future__ import annotations
 
@@ -316,6 +315,53 @@ def boundary_matrix(lo: torch.Tensor, hi: torch.Tensor, n: int, method: str = "q
     return mat
 
 
+def boundary_matrix_sparse(lo: torch.Tensor, hi: torch.Tensor, n: int, method: str = "qr") -> torch.Tensor:
+    """``boundary_matrix(lo, hi, n, method).to_sparse()`` assembled from its O(n L) entries: the same values, the same
+    orthogonalised boundary rows, without the dense [n, n] operator (34 GB of float64 at n = 65536)."""
+    L = lo.shape[0]
+    start = L // 2 - 1 + L % 2
+    r = torch.arange(1, n, 2) + start
+    m = r.shape[0]
+    cols = r.reshape(-1, 1) - torch.arange(L).reshape(1, -1)          # column of tap k in conv row i
+    valid = (cols >= 0) & (cols < n)
+    inner = valid.sum(1) == L
+    idx_i, idx_j, vals, sel = [], [], [], []
+    for b, filt in enumerate((lo, hi)):
+        taps = filt.reshape(1, -1).expand(m, L)
+        keep = valid & inner.reshape(-1, 1)
+        idx_i.append((torch.arange(m).reshape(-1, 1) + b * m).expand(m, L)[keep])
+        idx_j.append(cols[keep])
+        vals.append(taps[keep])
+        for i in (~inner).nonzero().reshape(-1).tolist():
+            row = torch.zeros(n, dtype=filt.dtype)
+            row[cols[i][valid[i]]] = filt[valid[i]]
+            sel.append((b * m + i, row))
+    if sel:
+        rows = torch.stack([row for _, row in sel])
+        if method == "qr":
+            q, _ = torch.linalg.qr(rows.T)
+            new = q.T
+        elif method == "gramschmidt":
+            new = rows.clone()
+            for p in range(new.shape[0]):
+                cur = new[p].clone()
+                acc = torch.zeros_like(cur)
+                for d in range(p):
+                    acc += torch.dot(cur, new[d]) * new[d]
+                cur = cur - acc
+                new[p] = cur / torch.linalg.vector_norm(cur)
+        else:
+            raise ValueError(f"Invalid orthogonalization method: {method}")
+        for (i, _), row in zip(sel, new):
+            nz = (row != 0).nonzero().reshape(-1)
+            idx_i.append(torch.full_like(nz, i))
+            idx_j.append(nz)
+            vals.append(row[nz])
+    i, j, v = torch.cat(idx_i), torch.cat(idx_j), torch.cat(vals)
+    nz = v != 0
+    return torch.sparse_coo_tensor(torch.stack([i[nz], j[nz]]), v[nz], (2 * m, n)).coalesce()
+
+
 def _odd_pad(x: torch.Tensor, mode: str) -> torch.Tensor:
     """One sample appended on the right of [B, n] (matmul_transform.py:381-388, 412-421)."""
     if mode not in _TORCH_MODE:
@@ -347,7 +393,7 @@ class MatrixWavedec:
             pad = cur % 2 != 0
             cur += 1 if pad else 0
             self.pads.append(pad)
-            self.ops.append(boundary_matrix(dec_lo, dec_hi, cur, self.method).to_sparse())
+            self.ops.append(boundary_matrix_sparse(dec_lo, dec_hi, cur, self.method))
             cur //= 2
 
     def __call__(self, data):
@@ -391,7 +437,7 @@ class MatrixWaverec:
             if cur < L:
                 break
             cur += cur % 2
-            self.ops.append(boundary_matrix(rec_lo, rec_hi, cur, self.method).T.to_sparse())
+            self.ops.append(boundary_matrix_sparse(rec_lo, rec_hi, cur, self.method).t().coalesce())
             cur //= 2
 
     def __call__(self, coeffs):

@@ -1,8 +1,8 @@
-"""pytorch_wavelet_toolbox_b200 -- B200-native backend for ptwt's fast wavelet transforms.
+"""pytorch_wavelet_toolbox_b200 -- H100-native backend for ptwt's fast wavelet transforms.
 
 The eight names below are drop-ins for the functions / classes of the same name in
 ``ptwt`` (v0lta/PyTorch-Wavelet-Toolbox): identical signatures, return containers and
-errors; the arithmetic runs in hand-written sm_100a CUDA kernels behind the C ABI declared
+errors; the arithmetic runs in hand-written sm_90a CUDA kernels behind the C ABI declared
 in ``include/wtb200.h``.
 
     import pytorch_wavelet_toolbox_b200 as ptwt_b200

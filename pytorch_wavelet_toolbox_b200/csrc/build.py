@@ -1,9 +1,9 @@
-"""Build libwtb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libwtb200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m pytorch_wavelet_toolbox_b200.csrc.build [--force] [--verbose]
 
 The shared object is plain C ABI (include/wtb200.h): no torch / pybind dependency, the
-CUDA runtime is linked statically, so the file built here runs unchanged on the GPU box.
+CUDA runtime is linked statically, so the file runs on any machine with an H100 and a recent driver.
 """
 from __future__ import annotations
 
@@ -39,7 +39,7 @@ def build(force: bool = False, verbose: bool = False, extra: list[str] | None = 
         return LIB
     cmd = [
         _nvcc(), "-O3", "-std=c++17",
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-lineinfo",
         "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
         "--expt-relaxed-constexpr",

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the B200 (sm_100a) wavelet filter bank.
+// common.cuh -- shared device helpers for the H100 (sm_90a) wavelet filter bank.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -13,8 +13,7 @@
 namespace wtb {
 
 // Opt a kernel in to `bytes` of dynamic shared memory.  cudaFuncSetAttribute is a driver call whose cost is far from
-// negligible when the value CHANGES from launch to launch (measured: ~1.3 ms per change, 4 ms of host time per
-// MatrixWavedec call in round 1), so the limit is only ever raised, once per (device, kernel), and kernels whose
+// negligible when the value CHANGES from launch to launch (milliseconds of host time per call), so the limit is only ever raised, once per (device, kernel), and kernels whose
 // need varies with the problem ask for their maximum up front.
 template <typename K>
 static cudaError_t ensure_dyn_smem(K kern, size_t bytes) {
@@ -31,6 +30,14 @@ static cudaError_t ensure_dyn_smem(K kern, size_t bytes) {
     return e;
 }
 constexpr size_t WTB_MAX_DYN_SMEM = 227 * 1024;
+
+// SM count of the current device (132 on an H100 SXM): the grid-size heuristics fill the machine with it.
+static inline int sm_count() {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 132;
+    return n;
+}
 
 
 // Filter taps travel as kernel parameters (no __constant__ symbols), so concurrent

@@ -1,4 +1,4 @@
-// fused2d.cuh -- 2-D analysis level as ONE kernel: rolling column strips on sm_100a.
+// fused2d.cuh -- 2-D analysis level as ONE kernel: rolling column strips on sm_90a.
 //
 // Replaces, per level, the reference's  F.pad -> conv2d(4 x [L x L], stride 2) -> split
 // (src/ptwt/conv_transform_2.py:142-149) by a separable polyphase filter bank that reads the
@@ -69,20 +69,16 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 }
 
 // ------------------------------------------------------------------------------------------
-// packed-FP32 filter helpers (FFMA2 = fma.rn.f32x2, one issue slot for two FMAs on sm_100a)
+// paired-FP32 filter helpers: taps and samples travel as float2 pairs (even / odd polyphase halves).
+// sm_90a has no packed FP32 FMA, so a pair is two round-to-nearest FMAs.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float2 ffma2(const float2 a, const float2 b, const float2 c) {
-    float2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;"
-        : "=l"(*reinterpret_cast<unsigned long long*>(&d))
-        : "l"(*reinterpret_cast<const unsigned long long*>(&a)), "l"(*reinterpret_cast<const unsigned long long*>(&b)),
-          "l"(*reinterpret_cast<const unsigned long long*>(&c)));
-    return d;
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 // Row filter of one thread: 8 consecutive (lo, hi) outputs from the register window v[].
 // out[g] = sum_k dec[L-1-k] v[2g+k+OFF], evaluated as an even-tap and an odd-tap partial sum in the
-// two halves of one FFMA2 accumulator.
+// two halves of one paired accumulator.
 template <int L, int OFF, int NV>
 __device__ __forceinline__ void row_filter8(const float (&v)[NV], const float2* __restrict__ pl,
                                             const float2* __restrict__ ph, float (&lo)[8], float (&hi)[8]) {
@@ -140,7 +136,7 @@ struct Fwd2dParams {
     int batch0;              // batch offset of this launch (gridDim.z chunking)
     int vec_store;           // 1: every output row start is 16-byte aligned -> 128-bit stores
     Taps<T> taps;            // un-flipped dec_lo / dec_hi
-    // float32 fast kernel: taps packed for FFMA2 (see row_filter8 / col_filter2x4)
+    // float32 fast kernel: taps packed in pairs (see row_filter8 / col_filter2x4)
     float2 pl[8], ph[8], bl[16], bh[16];
 };
 
@@ -148,8 +144,7 @@ template <int L, int TW, int ES = 4, int NSTAGE_ = 2>
 struct Fwd2dGeom {
     static constexpr int HALO = L - 2;
     // TMA needs the box to start on a 16-byte boundary: the staged tile begins HAL >= HALO columns
-    // left of the first output's window, HAL * ES a multiple of 16 (measured: a misaligned
-    // innermost coordinate traps with "illegal instruction" on sm_100a).
+    // left of the first output's window, HAL * ES a multiple of 16.
     static constexpr int HAL = ((HALO * ES + 15) / 16) * 16 / ES;
     static constexpr int OFF = HAL - HALO;        // columns skipped at the left of the tile
     static constexpr int CH = 16;                 // output rows per chunk
@@ -422,7 +417,7 @@ fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_consta
 }
 
 // ------------------------------------------------------------------------------------------
-// float32 fast variant: same structure as fwd2d_strip_kernel, with packed FP32 FMAs (FFMA2), mirror
+// float32 fast variant: same structure as fwd2d_strip_kernel, with paired FP32 taps (ffma2), mirror
 // rows behind the ring (column-pass windows never wrap, so their loads use immediate offsets) and
 // all per-thread index arithmetic hoisted out of the chunk loop.
 // ------------------------------------------------------------------------------------------
@@ -782,11 +777,9 @@ static int fused2d_fwd_try(int ndim, int mode, int levels, int L, const double* 
     // Chunking: the batch is cut into chunks that alternate between the caller's stream and one auxiliary
     // stream, so that the latency-bound deep levels of one chunk run under the bandwidth-bound level-1 launch
     // of the next.  The intermediate approximations cA_1 .. cA_{n-1} are scratch, so every chunk reuses the
-    // scratch slots of its stream.  (Small chunks would keep those slots L2-resident -- tools/l2_hint_probe
-    // shows that a <= 32 MB buffer written, read and overwritten in place survives any amount of streaming
-    // traffic on B200 -- but with one launch per level and chunk the launch tails cost more than the saved
-    // traffic: 64 chunks 2.80 ms, 16 chunks 2.03 ms, 2 chunks 1.89 ms; tools/ab_chunk.sh.  The persistent
-    // kernel in fused2d_mega.cuh is the way to use that effect.)
+    // scratch slots of its stream.  (Small chunks could keep those slots L2-resident, but with one launch per
+    // level and chunk the launch tails grow with the chunk count; the persistent kernel in fused2d_mega.cuh is
+    // the way to try that effect.)
     int64_t chunk = 0;   // images per chunk
     int nstreams = 2;
     if (knob_is_set(K_CHUNK)) chunk = knob_val(K_CHUNK, 0);

@@ -7,15 +7,13 @@
 //
 //     period p :  level-1 items of image p, level-2 items of image p-1, level-3 items of image p-2, ...
 //
-// The idea was that cA_1 of an image, consumed one period (~20 us) after it was produced, would still be
-// resident in the 126 MB L2.  MEASURED (profiles/r01_mega_*, tools/ncu_mega_ring.sh): it is not -- DRAM
-// traffic stays at 5.7 GB read + 5.7 GB written per 64-image step whether the L2 cache hints
-// (evict_first for streaming loads / detail stores, evict_last for approximation stores) are on or off
-// and whether or not the approximations are confined to a ring of 2-4 reused scratch slots
-// (WTB200_MEGA_RING) -- and the kernel is 10 % slower than the per-level launches.  It is kept because the
-// scheduling machinery (queue, completion counters, write-after-read protection of the slot ring, TMA
-// reads of data produced by other SMs) is correct, tested in every boundary mode, and the starting point
-// for whatever keeps cA on chip next.
+// The idea is that cA_1 of an image, consumed one period after it was produced, is still resident in L2
+// (50 MB on an H100), optionally helped by L2 cache hints (evict_first for streaming loads / detail
+// stores, evict_last for approximation stores) and by a ring of 2-4 reused scratch slots
+// (WTB200_MEGA_RING).  With hundreds of resident CTAs the in-flight window is larger than L2, so the
+// per-level launches stay the default.  The scheduling machinery (queue, completion counters,
+// write-after-read protection of the slot ring, TMA reads of data produced by other SMs) is correct,
+// tested in every boundary mode, and the starting point for whatever keeps cA on chip next.
 //
 //   * persistent CTAs (3 per SM) fetch item indices from a global atomic counter; an item of level l+1
 //     waits (ld.acquire spin by one thread) until the per-(level, image) completion counter of level l
@@ -387,9 +385,8 @@ static int launch_fwd2d_mega(int mode, int levels, const double* dlo, const doub
     const size_t smem = Fwd2dGeomF<L, 64>::SMEM;
     e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute");
-    int dev = 0, sms = 148, occ = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
+    int occ = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, smem);
     if (e != cudaSuccess || occ < 1) return 0;
     kern<<<sms * occ, 256, smem, st>>>(p, maps);

@@ -37,7 +37,7 @@ struct Pair2dParams {
     int mode;
     int batch0;
     int vec1, vec2;          // 128-bit stores allowed for level-1 details / level-2 bands
-    // filter taps packed for FFMA2 (fma.rn.f32x2): polyphase pairs for the row passes,
+    // filter taps packed in pairs for ffma2: polyphase pairs for the row passes,
     // broadcast pairs for the column passes (index j = tap applied to ring row j of the window)
     float2 pl[8], ph[8];     // {dec[L-1-2m], dec[L-2-2m]}
     float2 bl[16], bh[16];   // {dec[L-1-j], dec[L-1-j]}

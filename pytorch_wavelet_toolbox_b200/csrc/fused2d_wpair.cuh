@@ -13,7 +13,7 @@
 //     the warp's own mbarriers; the warp that consumed a stage re-arms it;
 //   * row pass: each lane slides the L taps over its 16-sample window (4 LDS.128 per row);
 //   * column pass WITHOUT a shared-memory ring: every pair of input rows is scattered into the L/2
-//     output rows it contributes to, held as FFMA2 accumulators in registers
+//     output rows it contributes to, held as paired (float2) accumulators in registers
 //     (acc[i] += dec[2(i-k)+1] * row[2k] + dec[2(i-k)] * row[2k+1]); one output row completes per
 //     pair and goes straight to HBM (three detail bands, 128-bit stores, 512 contiguous bytes/warp);
 //   * the completed approximation row goes to a two-row buffer in shared memory (the only exchange
@@ -481,7 +481,7 @@ static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_
         const int forced = (int)knob_val(K_WPAIR_SEG, 0);
         int big = forced > 0 ? forced : 144;
         // enough tasks to fill the machine a few times
-        const int64_t want = 3 * 148 * 12;
+        const int64_t want = 3 * (int64_t)sm_count() * 12;
         while (forced <= 0 && big > 32 && (int64_t)((p.Mh2 + big - 1) / big) * nstrip * B < want) big -= 16;
         int y = 0, n = 0;
         p.seg_start[0] = 0;
@@ -522,11 +522,8 @@ template <>
 bool try_wpair<float>(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
                       const wt_level& l2, int L, int mode, const Taps<float>& taps, cudaStream_t st,
                       uint64_t* launches, cudaError_t* err) {
-    // Opt-in (WTB200_WPAIR=1 / wt_set_knob("WPAIR", 1)): parity green, 19 % less DRAM traffic than one launch per level,
-    // but issue-bound (1.7 IPC/SM at 12 independent warps per SM) -- 1.84 ms vs 1.78-1.85 ms for the first two levels
-    // of 64 x 4096^2, i.e. no faster (profiles/r02_wpair_*).  Running it on part of the batch concurrently with the
-    // per-level kernels on the rest (different bottlenecks) was measured too: 2.01-2.08 ms vs 1.87 ms
-    // (profiles/r02_ab_wpair_hybrid.json).
+    // Opt-in (WTB200_WPAIR=1 / wt_set_knob("WPAIR", 1)): parity green and less DRAM traffic than one launch per
+    // level (cA1 never reaches HBM), but bound by instruction issue rather than by bytes, so it is not the default.
     if (!knob_on(K_WPAIR) || knob_on(K_NO_WPAIR) || knob_on(K_DISABLE_FUSED)) return false;
     switch (L) {
         case 2: return launch_fwd2d_wpair_t<2, 3, 12>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches, err);

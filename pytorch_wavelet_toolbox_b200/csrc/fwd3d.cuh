@@ -347,7 +347,7 @@ static cudaError_t launch_fwd3d_level(const float* x, int64_t B, int D, int H, i
         p.dh[j] = j < L ? p.bh[j] : make_float2(0.f, 0.f);
     }
     // tile shape: 16 x 32 unless another shape stages at least 25 % fewer input elements per plane
-    // (narrow or short planes; on 131 x 131 planes 11 x 44 stages 21 % fewer and measures no faster)
+    // (narrow or short planes)
     static const int shapes[3][2] = {{16, 32}, {11, 44}, {8, 64}};
     int best = 0;
     int64_t cost[3];

@@ -15,7 +15,7 @@
 //   * row pass (synthesis along W): lane <-> (band pair, coefficient row), warp <-> 16 output columns;
 //     (ll, hl) -> Lh and (lh, hh) -> Hh, written to a ring of 16 + L/2 - 1 rows (+ mirror rows);
 //   * column pass (synthesis along H): thread <-> (4 output rows, 4 output columns): L/2 + 1 ring rows
-//     of Lh and Hh (LDS.128, no wrap), 64 FFMA2, 4 coalesced STG.128.
+//     of Lh and Hh (LDS.128, no wrap), 64 paired FMAs (ffma2), 4 coalesced STG.128.
 //
 // Algorithmic bytes per level: 4 B * (4 Mh Mw read + OH OW written).
 #pragma once
@@ -34,7 +34,7 @@ struct Inv2dParams {
     int batch0;
     int vec_store;
     float rlo[16], rhi[16];  // un-flipped rec_lo / rec_hi (row pass, scalar FMAs)
-    float2 bl[16], bh[16];   // {rec_lo[k], rec_lo[k]}, {rec_hi[k], rec_hi[k]} (column pass, FFMA2)
+    float2 bl[16], bh[16];   // {rec_lo[k], rec_lo[k]}, {rec_hi[k], rec_hi[k]} (column pass, ffma2)
 };
 
 struct Inv2dMaps {

@@ -10,7 +10,7 @@
 
 namespace wtb {
 
-// Matrix FWT (matrix_dmma.cuh, matrix_fused.cuh; defaults from tools/ab_matrix2.py / tools/ab_matrix_inv.py):
+// Matrix FWT (matrix_dmma.cuh, matrix_fused.cuh):
 //   NO_DMMA          float64 without the FP64 tensor-core cascades (scalar fused / per-level kernels)
 //   MATF_VARIANT     1 = streaming DMMA analysis kernel instead of the polyphase one
 //   MATF_K / MATI_K  levels per launch (analysis / synthesis);  MATF_KCOARSE the same for rows <= 8192 samples

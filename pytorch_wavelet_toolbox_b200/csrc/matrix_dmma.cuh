@@ -8,10 +8,10 @@
 //
 //     D[8 x 8] = A[8 x (L+6)] * B[(L+6) x 8],   A[(band, s)][u] = f_band[u - 2 s],   B[u][g] = x[2 i0 + 8 g - HL + u]
 //
-// evaluated with mma.sync.aligned.m8n8k4.f64 (DMMA; tcgen05 has no f64 kind): about (L+6)/4 instructions of 256 FMAs
-// for 64 outputs.  60 % of those FMAs multiply structural zeros of A -- the price of the dense form -- but the kernel
-// is bound by instruction issue, not by the FP64 pipe (profiles/r02_matfwd_stream_ncu_summary.txt: DFMA 25 % of 214 M
-// warp instructions, fp64 pipe 22 % busy), and the DMMA form needs ~0.3 warp instructions per output instead of 1.5.
+// evaluated with mma.sync.aligned.m8n8k4.f64 (DMMA, the FP64 tensor-core instruction of sm_90; wgmma has no f64
+// kind): about (L+6)/4 instructions of 256 FMAs for 64 outputs.  60 % of those FMAs multiply structural zeros of A --
+// the price of the dense form -- but the scalar kernel is bound by instruction issue, not by the FP64 pipe, and the
+// DMMA form needs ~0.3 warp instructions per output instead of 1.5.
 //
 // Everything around the contraction is the streaming cascade of matrix_fused.cuh: a CTA takes consecutive chunks of one
 // row through K levels, level inputs live in shared memory (interleaved, as the B fragment wants them), the next chunk
@@ -274,7 +274,7 @@ static bool launch_mat_fwd_dmma(int L, int k, const int64_t* n, const int32_t* n
     const int nchunks = (nk + tk - 1) / tk;
     int cpc = (int)knob_val(K_MATF_CPC, 8);
     if (cpc < 1) cpc = 1;
-    const int64_t min_ctas = knob_val(K_MATF_MINCTAS, 4 * 148);
+    const int64_t min_ctas = knob_val(K_MATF_MINCTAS, 4 * sm_count());
     while (cpc > 1 && (int64_t)((nchunks + cpc - 1) / cpc) * batch < min_ctas) cpc /= 2;
     p.cpc = cpc;
     dim3 grid((nchunks + cpc - 1) / cpc, (unsigned)batch);
@@ -303,8 +303,8 @@ static bool launch_mat_fwd_dmma(int L, int k, const int64_t* n, const int32_t* n
 
 
 // ==========================================================================================
-// The analysis cascade again, laid out like the synthesis kernel below (which reaches 81 % of the HBM peak on its
-// finest launch where the kernel above reaches 64 %): one chunk per CTA, every level input kept as two POLYPHASE arrays
+// The analysis cascade again, laid out like the synthesis kernel below (conflict-free polyphase operand loads, which
+// the kernel above lacks): one chunk per CTA, every level input kept as two POLYPHASE arrays
 // (even samples | odd samples, the odd array two doubles further in the bank pattern), the DATA in the A operand and
 // the polyphase FILTER matrix in the B operand:
 //
@@ -800,8 +800,7 @@ __global__ void __launch_bounds__(NT) mat_inv_dmma_kernel(const __grid_constant_
 // The same cascade, streaming ROWS: a CTA keeps its chunk index and walks p.rows batch rows.  The coefficient ranges
 // and tile ranges depend on the chunk only, so they are computed once; the next row's details and coarsest
 // approximation arrive by TMA bulk copies (cp.async.bulk, one mbarrier per level and buffer set) while the current row
-// is synthesised, which removes the per-thread staging loops (19 % of the instructions of the kernel above,
-// profiles/r02_matinv_dmma_ncu_summary.txt) and the per-level range arithmetic (24 %).
+// is synthesised, which removes the per-thread staging loops and the per-level range arithmetic of the kernel above.
 // Needs 16-byte aligned rows and even band lengths (bulk copies move multiples of 16 bytes).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void md_mbar_init(uint64_t* bar, uint32_t count) {
@@ -1062,7 +1061,7 @@ static bool launch_mat_inv_dmma(int L, int k, const int64_t* n, int64_t keep0, c
     }
     p.vec = vec;
     for (int q = 0; q < L; ++q) { p.rlo[q] = rlo[q]; p.rhi[q] = rhi[q]; }
-    int chunk = 2048;                                               // tools/ab_matrix_inv.py
+    int chunk = 2048;
     if (knob_is_set(K_MATI_CHUNK)) { const int v = (int)knob_val(K_MATI_CHUNK, 0); if (v >= 64 && v <= 16384) chunk = v; }
     if (!knob_is_set(K_MATI_CHUNK)) {
         // short rows: smaller chunks until the launch has MATI_MINCTAS CTAs
@@ -1095,7 +1094,7 @@ static bool launch_mat_inv_dmma(int L, int k, const int64_t* n, int64_t keep0, c
     if (forced) rows = -rows;
     if (rows > 64) rows = 64;
     if (!forced)
-        while (rows > 1 && (int64_t)nchunks * ((batch + rows - 1) / rows) < 8 * 148) rows /= 2;
+        while (rows > 1 && (int64_t)nchunks * ((batch + rows - 1) / rows) < 8 * sm_count()) rows /= 2;
     p.rows = rows; p.batch = (int)batch; p.cap_lo = len;           // len = capacity of the coarsest range
     const size_t smem_rows = (size_t)(2 * cap + 2 * len + 2 * hcap + 4) * sizeof(double);
     if (rows_ok && rows >= 1 && smem_rows <= 200 * 1024 && batch < (int64_t(1) << 31)) {

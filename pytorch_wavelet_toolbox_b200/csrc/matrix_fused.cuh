@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(NT, MINB) mat_fwd_fused_kernel(const __grid_co
     const T* __restrict__ xb = p.x + (int64_t)b * p.x_stride;
 
     // A CTA streams `cpc` consecutive chunks of one row: while chunk c is taken through the K levels, the samples of
-    // chunk c + 1 travel into `raw` with cp.async (round 1 staged, synchronised and only then computed: 28 %).
+    // chunk c + 1 travel into `raw` with cp.async.
     // ranges: rlo[j], rhi[j] = level-j indices this CTA computes (j >= 1) / stages (j = 0) for one chunk; two sets in
     // shared memory (current chunk / prefetched chunk).  In registers the run-time level index costs a local array.
     __shared__ int s_r[2][2][MATF_MAXK + 1];
@@ -282,7 +282,7 @@ static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* 
     p.lo = lo_out; p.lo_stride = lo_stride;
     for (int q = 0; q < L; ++q) { p.flo[q] = taps.lo[L - 1 - q]; p.fhi[q] = taps.hi[L - 1 - q]; }
     const int nk = p.n[k];
-    int chunk0 = sizeof(T) == 8 ? 2048 : 4096;                    // level-0 samples per chunk (tools/ab_matrix2.py)
+    int chunk0 = sizeof(T) == 8 ? 2048 : 4096;                    // level-0 samples per chunk
     if (knob_is_set(K_MATF_CHUNK)) { const int v = (int)knob_val(K_MATF_CHUNK, 0); if (v >= 64 && v <= 16384) chunk0 = v; }
     if (n[0] <= 8192 && n[0] > chunk0) chunk0 = (int)n[0];        // short rows: the whole row is one chunk
     int tk = chunk0 >> k;
@@ -299,11 +299,11 @@ static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* 
     const int nchunks = (nk + tk - 1) / tk;
     int cpc = (int)knob_val(K_MATF_CPC, 8);
     if (cpc < 1) cpc = 1;
-    while (cpc > 1 && (int64_t)((nchunks + cpc - 1) / cpc) * batch < 4 * 148) cpc /= 2;   // keep the machine full
+    while (cpc > 1 && (int64_t)((nchunks + cpc - 1) / cpc) * batch < 4 * sm_count()) cpc /= 2;   // keep the machine full
     p.cpc = cpc;
     dim3 grid((nchunks + cpc - 1) / cpc, (unsigned)batch);
     // CTA shape: 128 threads for small chunks (more CTAs per SM: the staging loads of one overlap the cascade of the
-    // others), 256 for large ones.  MATF_NT / MATF_MINB override (tools/ab_matrix.py).
+    // others), 256 for large ones.  MATF_NT / MATF_MINB override.
     int nt = chunk0 <= 2048 ? 128 : 256;
     if (knob_is_set(K_MATF_NT)) nt = knob_val(K_MATF_NT, 256) == 128 ? 128 : 256;
     const int minb = (int)knob_val(K_MATF_MINB, 1);

@@ -1,5 +1,5 @@
-// wtb200.cu -- C ABI (include/wtb200.h) and host-side drivers of the B200 wavelet
-// filter bank.  Build: see build.py (nvcc -gencode arch=compute_100a,code=sm_100a).
+// wtb200.cu -- C ABI (include/wtb200.h) and host-side drivers of the H100 wavelet
+// filter bank.  Build: see build.py (nvcc -gencode arch=compute_90a,code=sm_90a).
 //
 // Host drivers here only sequence launches; they never allocate device memory, never
 // synchronise, and keep no state besides the launch counter and the thread-local error
@@ -66,7 +66,7 @@ static inline int64_t coeff_len(int64_t n, int L) {
 
 static int grid_for(int64_t total, int block) {
     int64_t g = (total + block - 1) / block;
-    const int64_t cap = 148LL * 64;  // grid-stride beyond this
+    const int64_t cap = (int64_t)sm_count() * 64;  // grid-stride beyond this
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;
@@ -557,9 +557,8 @@ static int matrix_fwd_t(int levels, int L, const double* dlo, const double* dhi,
             // group of consecutive unpadded levels -> one fused launch
             int k = 0;
             // float32: 4 levels per launch while a row is cut into chunks, all remaining levels (up to MATF_MAXK) once
-            // a whole row fits one chunk (tools/ab_matrix2.py).  float64 (DMMA cascade): 2 levels per launch throughout
-            // -- config 4: 0.355 ms against 0.411 / 0.381 with 3 / 4 and 0.372 with one launch for the short rows
-            // (tools/ab_matrix_inv.py)
+            // a whole row fits one chunk.  float64 (DMMA cascade): 2 levels per launch throughout (deeper cascades
+            // save traffic but lose more to CTA barriers and thin coarse levels)
             const bool dmma64 = sizeof(T) == 8 && !knob_on(K_NO_DMMA);
             int kmax = n[l] <= 8192 ? (int)knob_val(K_MATF_KCOARSE, dmma64 ? 2 : MATF_MAXK) : (dmma64 ? 2 : 4);
             if (kmax < 1 || kmax > MATF_MAXK) kmax = MATF_MAXK;
@@ -678,10 +677,9 @@ static int matrix_inv_t(int levels, int L, const double* rlo, const double* rhi,
         if (allow_fused && !knob_on(K_DISABLE_FUSED)) {
             // group of levels l, l-1, ..., l-k+1 whose intermediate results are not trimmed -> one launch.
             // float64: the synthesis cascade on the FP64 tensor cores (matrix_dmma.cuh), 2 levels per launch -- deeper
-            // cascades save HBM traffic but lose more to barriers and thin coarse levels (config 4: 0.316 ms with 2,
-            // 0.386 with 3, 0.366 with 4 levels per launch, 0.336 with 2 + one launch for all levels whose row fits
-            // a CTA; tools/ab_matrix_inv.py).  float32: per-level kernels by default -- the scalar fused synthesis
-            // kernel (0.79 ms) is slower than twelve register-blocked per-level launches (0.57 ms).
+            // cascades save HBM traffic but lose more to barriers and thin coarse levels.  float32: per-level kernels
+            // by default -- the scalar fused synthesis kernel reads shared memory with 2-way bank conflicts and
+            // synchronises once per level, the register-blocked per-level kernels do neither.
             // WTB200_MATI_K sets the number of levels per launch for both.
             const bool dmma = sizeof(T) == 8 && !knob_on(K_NO_DMMA);
             int kmax = dmma ? 2 : 1;

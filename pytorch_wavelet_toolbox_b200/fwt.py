@@ -1,4 +1,4 @@
-"""Padded multi-level fast wavelet transform in 1, 2 and 3 dimensions on B200.
+"""Padded multi-level fast wavelet transform in 1, 2 and 3 dimensions on the H100.
 
 Drop-in for ``ptwt.wavedec / waverec`` (``/root/reference/src/ptwt/conv_transform.py:69,146``),
 ``ptwt.wavedec2 / waverec2`` (``conv_transform_2.py:74,160``) and ``ptwt.wavedec3 / waverec3``
@@ -56,7 +56,7 @@ def _compute_device(t: torch.Tensor) -> torch.device:
         raise RuntimeError(f"unsupported device {t.device}; expected a CUDA or CPU tensor")
     if not torch.cuda.is_available():
         raise RuntimeError(
-            "pytorch_wavelet_toolbox_b200 needs a CUDA device (B200, sm_100a): the transforms have "
+            "pytorch_wavelet_toolbox_b200 needs a CUDA device (H100, sm_90a): the transforms have "
             "no CPU implementation. Got a CPU tensor and torch.cuda.is_available() is False."
         )
     return torch.device("cuda", torch.cuda.current_device())

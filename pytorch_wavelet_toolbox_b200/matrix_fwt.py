@@ -1,4 +1,4 @@
-"""Boundary-filter ("matrix") fast wavelet transform on B200.
+"""Boundary-filter ("matrix") fast wavelet transform on the H100.
 
 Drop-in for ``ptwt.MatrixWavedec`` / ``ptwt.MatrixWaverec``
 (``/root/reference/src/ptwt/matmul_transform.py:172,502``).  The reference materialises one

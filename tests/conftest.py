@@ -17,7 +17,7 @@ GOLDEN = ROOT / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
     config.addinivalue_line("markers", "slow: long-running")
 
 
@@ -34,6 +34,14 @@ def pytest_collection_modifyitems(config, items):
 def golden():
     manifest = json.loads((GOLDEN / "reference_vectors.json").read_text())
     arrays = np.load(GOLDEN / "reference_vectors.npz")
+    return manifest, arrays
+
+
+@pytest.fixture(scope="session")
+def reference_api():
+    """What the unmodified reference computed beyond the transform vectors (oracle/make_golden_api.py)."""
+    manifest = json.loads((GOLDEN / "reference_api.json").read_text())
+    arrays = np.load(GOLDEN / "reference_api.npz")
     return manifest, arrays
 
 

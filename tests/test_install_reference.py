@@ -1,101 +1,65 @@
-"""install() / uninstall() against the REAL reference package (baseline/_ref, placed by baseline/make_ref.py in the build
-container; it travels to the GPU box with the snapshot): rebinding in ptwt and in the modules that captured the names by
-value, the reference's own packet classes and learnable filters running on the new kernels."""
+"""install() / uninstall() on a package with the reference's module layout (tests/stand_in_ptwt.py): rebinding in ptwt
+and in the modules that captured the names by value, and the numbers and gradients of the unmodified reference
+(stored by oracle/make_golden_api.py) reproduced by the new kernels."""
 from __future__ import annotations
 
 import pytest
 import torch
 
 import pytorch_wavelet_toolbox_b200 as wt
+from conftest import flatten_coeffs
+from stand_in_ptwt import stand_in_ptwt
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture
 def ptwt():
-    from baseline.make_ref import import_ref
-
-    mod = import_ref()
-    if mod is None:
-        pytest.skip("baseline/_ref is not present (python baseline/make_ref.py in the build container)")
-    yield mod
-    wt.uninstall()
+    with stand_in_ptwt() as mod:
+        yield mod
 
 
-def test_install_rebinds_and_uninstall_restores(ptwt):
-    import ptwt.packets as packets
-    import ptwt.separable_conv_transform as sep
-
+def test_install_rebinds_and_uninstall_restores(ptwt, reference_api):
+    packets, sep = ptwt.packets, ptwt.separable_conv_transform
+    manifest, arrays = reference_api
     ref_wavedec, ref_packets_wavedec, ref_sep_wavedec = ptwt.wavedec, packets.wavedec, sep.wavedec
     replaced = wt.install()
     assert "ptwt.wavedec" in replaced and "ptwt.packets.wavedec" in replaced
     assert ptwt.wavedec is wt.wavedec and packets.wavedec is wt.wavedec and sep.wavedec is wt.wavedec
     assert ptwt.conv_transform_2.wavedec2 is wt.wavedec2 and ptwt.matmul_transform.MatrixWavedec is wt.MatrixWavedec
-    x = torch.randn(2, 3, 64, 48, device="cuda")
+    assert ptwt.WaveletPacket is wt.WaveletPacket and packets.WaveletPacket2D is wt.WaveletPacket2D
+    x = torch.from_numpy(arrays["install_x"]).cuda()
     got = ptwt.wavedec2(x, "db2", level=2)                      # the reference's name, our kernels
     wt.uninstall()
     assert ptwt.wavedec is ref_wavedec and packets.wavedec is ref_packets_wavedec and sep.wavedec is ref_sep_wavedec
-    want = ptwt.wavedec2(x.cpu(), "db2", level=2)               # the reference itself on the CPU
-    flat = lambda c: [c[0]] + [b for lv in c[1:] for b in lv]   # noqa: E731
-    scale = max(float(t.abs().max()) for t in flat(want))
-    for a, b in zip(flat(got), flat(want)):
+    want = [torch.from_numpy(arrays[f"install_o{j}"]) for j in range(manifest["install_n_out"])]
+    scale = max(float(t.abs().max()) for t in want)
+    flat = flatten_coeffs(got)
+    assert len(flat) == len(want)
+    for a, b in zip(flat, want):
         assert a.is_cuda and float((a.cpu() - b).abs().max()) <= 1e-5 * scale
 
 
-def test_reference_packet_classes_ride_on_the_installed_kernels(ptwt):
-    """The reference's own WaveletPacket captured wavedec by value (packets.py:34-37): after install() it runs every node
-    through our level-1 kernels and still produces the reference's numbers."""
-    import ptwt.packets as packets
-
-    ref_cls = packets.WaveletPacket
-    x = torch.randn(3, 128, dtype=torch.float64)
-    want = ref_cls(x, "db3", mode="reflect", maxlevel=3)
-    keys = want.get_level(3)
-    want_nodes = {k: want[k] for k in keys}
-    wt.install()
-    assert packets.wavedec is wt.wavedec
-    got = ref_cls(x.cuda(), "db3", mode="reflect", maxlevel=3)   # the reference's class, not ours
-    scale = max(float(t.abs().max()) for t in want_nodes.values())
-    for k in keys:
-        assert got[k].is_cuda and float((got[k].cpu() - want_nodes[k]).abs().max()) <= 1e-11 * scale
-    ours = ptwt.WaveletPacket(x.cuda(), "db3", mode="reflect", maxlevel=3)   # rebound to the batched class
-    assert type(ours) is wt.WaveletPacket
-    ours.initialize(keys)
-    for k in keys:
-        assert float((ours[k].cpu() - want_nodes[k]).abs().max()) <= 1e-11 * scale
-
-
-def test_reference_learnable_filters_train_through_the_installed_backend(ptwt):
-    """ptwt.wavelets_learnable.ProductFilter (nn.Parameters behind filter_bank, wavelets_learnable.py:167-199) through
-    ptwt.wavedec / waverec after install(): the four filters and the data receive the reference's gradients
-    (the pattern of examples/network_compression/wavelet_linear.py:118,150)."""
-    from ptwt.wavelets_learnable import ProductFilter
-
-    def make():
-        fb = wt.WaveletTensorTuple.from_wavelet(wt._wavelets.as_wavelet("db3"), torch.float64)
-        return ProductFilter(*[t.clone() for t in fb])
-
-    g = torch.Generator().manual_seed(3)
-    x = torch.randn(4, 96, generator=g, dtype=torch.float64)
-    w = torch.randn(4, 96, generator=g, dtype=torch.float64)
-
-    def loss_of(mod, wav, data, weight):
-        c = mod.wavedec(data, wav, level=3, mode="reflect")
-        rec = mod.waverec(c, wav)[..., :96]
-        return sum((t * t).sum() for t in c) + (rec * weight).sum() + wav.wavelet_loss()
-
-    ref_wav = make()
-    xr = x.clone().requires_grad_(True)
-    loss_ref = loss_of(ptwt, ref_wav, xr, w)
-    loss_ref.backward()
-    wt.install()
-    our_wav = make()
+def test_learnable_filters_receive_the_reference_gradients(reference_api):
+    """Filter taps as nn.Parameters (the reference's learnable ProductFilter, wavelets_learnable.py:167-199, trained
+    through wavedec / waverec as in examples/network_compression/wavelet_linear.py:118,150): the loss, the data and
+    the four filters receive the gradients the reference computed."""
+    manifest, arrays = reference_api
+    spec = manifest["learnable"]
+    fb = wt.WaveletTensorTuple.from_wavelet(wt._wavelets.as_wavelet(spec["wavelet"]), torch.float64)
+    wav = wt.WaveletTensorTuple(*[torch.nn.Parameter(t.clone()) for t in fb])
+    x = torch.from_numpy(arrays["learn_x"])
+    w = torch.from_numpy(arrays["learn_w"])
+    n = x.shape[-1]
     xo = x.clone().cuda().requires_grad_(True)
-    loss_our = loss_of(ptwt, our_wav, xo, w.cuda())
-    loss_our.backward()
-    assert abs(float(loss_our) - float(loss_ref)) <= 1e-10 * abs(float(loss_ref))
-    assert float((xo.grad.cpu() - xr.grad).abs().max()) <= 1e-10 * float(xr.grad.abs().max())
+    c = wt.wavedec(xo, wav, level=spec["level"], mode=spec["mode"])
+    rec = wt.waverec(c, wav)[..., :n]
+    loss = sum((t * t).sum() for t in c) + (rec * w.cuda()).sum()
+    loss.backward()
+    assert abs(float(loss) - spec["loss"]) <= 1e-10 * abs(spec["loss"])
+    want = torch.from_numpy(arrays["learn_grad_x"])
+    assert float((xo.grad.cpu() - want).abs().max()) <= 1e-10 * float(want.abs().max())
     for name in ("dec_lo", "dec_hi", "rec_lo", "rec_hi"):
-        a, b = getattr(our_wav, name).grad, getattr(ref_wav, name).grad
+        a, b = getattr(wav, name).grad, torch.from_numpy(arrays[f"learn_grad_{name}"])
         assert a is not None, name
-        assert float((a - b).abs().max()) <= 1e-9 * float(b.abs().max()), name
+        assert float((a.cpu() - b).abs().max()) <= 1e-9 * float(b.abs().max()), name

@@ -16,7 +16,7 @@ import pytorch_wavelet_toolbox_b200 as wt
 from conftest import GOLDEN, assert_close_rel
 
 
-def test_orders_match_the_reference_definitions():
+def test_orders_match_the_reference_definitions(reference_api):
     assert wt.WaveletPacket.get_level(0) == [""]
     assert wt.WaveletPacket.get_level(2) == ["aa", "ad", "dd", "da"]                       # Gray code
     assert wt.WaveletPacket.get_level(2, "natural") == ["aa", "ad", "da", "dd"]
@@ -28,14 +28,12 @@ def test_orders_match_the_reference_definitions():
     assert wt.WaveletPacket2D.get_freq_order(1) == [["a", "v"], ["h", "d"]]
     f2 = wt.WaveletPacket2D.get_freq_order(2)
     assert [len(r) for r in f2] == [4, 4, 4, 4] and f2[0][0] == "aa" and sorted(sum(f2, [])) == sorted(nat)
-    from oracle.ref_import import import_reference, reference_available
-    if reference_available():
-        ptwt = import_reference()
-        for lev in (0, 1, 2, 3):
-            assert wt.WaveletPacket.get_level(lev) == ptwt.WaveletPacket.get_level(lev)
-            assert wt.WaveletPacket.get_level(lev, "natural") == ptwt.WaveletPacket.get_level(lev, "natural")
-            assert wt.WaveletPacket2D.get_freq_order(lev) == ptwt.WaveletPacket2D.get_freq_order(lev)
-            assert wt.WaveletPacket2D.get_natural_order(lev) == ptwt.WaveletPacket2D.get_natural_order(lev)
+    ref = reference_api[0]["packet_orders"]            # the unmodified reference's orders (oracle/make_golden_api.py)
+    for lev in (0, 1, 2, 3):
+        assert wt.WaveletPacket.get_level(lev) == ref[str(lev)]["level"]
+        assert wt.WaveletPacket.get_level(lev, "natural") == ref[str(lev)]["level_natural"]
+        assert wt.WaveletPacket2D.get_freq_order(lev) == ref[str(lev)]["freq_2d"]
+        assert wt.WaveletPacket2D.get_natural_order(lev) == ref[str(lev)]["natural_2d"]
 
 
 def test_access_errors_without_touching_the_device():
