@@ -140,7 +140,7 @@ struct Fwd2dParams {
     float2 pl[8], ph[8], bl[16], bh[16];
 };
 
-template <int L, int TW, int ES = 4, int NSTAGE_ = 2>
+template <int L, int TW, int ES = 4>
 struct Fwd2dGeom {
     static constexpr int HALO = L - 2;
     // TMA needs the box to start on a 16-byte boundary: the staged tile begins HAL >= HALO columns
@@ -153,7 +153,7 @@ struct Fwd2dGeom {
     static constexpr int SW = ((NEED - 4 + 7) / 8) * 8 + 4;  // smem pitch: >= NEED, == 4 (mod 8)
     static constexpr int MP = TW + 4;             // pitch of the row-filtered ring (== 4 mod 8 for TW % 8 == 0)
     static constexpr int RING = IN_ROWS + HALO;   // ring rows: one chunk plus the vertical halo
-    static constexpr int NSTAGE = NSTAGE_;
+    static constexpr int NSTAGE = 2;              // input stages: one being filtered, one in flight
     static constexpr int G = 8;                   // output columns per thread in the row pass
     static constexpr int NWARP = TW / G;
     static constexpr int NTHREADS = 32 * NWARP;
@@ -174,11 +174,10 @@ template <typename T> struct VecOf;
 template <> struct VecOf<float> { using type = float4; };
 template <> struct VecOf<double> { using type = double2; };
 
-template <typename T, int L, int TW, bool USE_TMA, int NSTG = 2>
-__global__ void __launch_bounds__((Fwd2dGeom<L, TW, sizeof(T), NSTG>::NTHREADS),
-                                  (sizeof(T) == 4 && NSTG == 2 ? (TW == 64 ? 4 : 6) : 2))
+template <typename T, int L, int TW, bool USE_TMA>
+__global__ void __launch_bounds__((Fwd2dGeom<L, TW, sizeof(T)>::NTHREADS), (sizeof(T) == 4 ? 4 : 2))
 fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_constant__ CUtensorMap tmap) {
-    using Gm = Fwd2dGeom<L, TW, sizeof(T), NSTG>;
+    using Gm = Fwd2dGeom<L, TW, sizeof(T)>;
     using V = typename VecOf<T>::type;
     constexpr int OFF = Gm::OFF, HAL = Gm::HAL;
     constexpr int HALO = Gm::HALO, CH = Gm::CH, IN_ROWS = Gm::IN_ROWS, SW = Gm::SW, MP = Gm::MP;
@@ -213,11 +212,8 @@ fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_consta
         }
         __syncthreads();
         if (tid == 0) {
-            // NSTAGE == 2: both stages are filled up front and a stage is refilled once its chunk has
-            // been row-filtered.  NSTAGE > 2: NSTAGE-1 loads stay in flight all the time -- the load of
-            // chunk c + NSTAGE - 1 is issued at the top of iteration c into the stage chunk c - 1 used.
-            constexpr int PRE = NSTAGE == 2 ? 2 : NSTAGE - 1;
-            for (int s = 0; s < PRE && s < nchunks; ++s) {
+            // both stages are filled up front; a stage is refilled once its chunk has been row-filtered
+            for (int s = 0; s < NSTAGE && s < nchunks; ++s) {
                 mbar_expect_tx(&bars[s], (uint32_t)Gm::stage_bytes(sizeof(T)));
                 tma_load_3d(s_in + (size_t)s * IN_ROWS * SW, &tmap, &bars[s], c_in0, r_in0 + s * IN_ROWS, b);
             }
@@ -236,12 +232,6 @@ fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_consta
         const int r_base = r_in0 + c * IN_ROWS;     // absolute input row of tile row 0
 
         if (USE_TMA) {
-            if (NSTAGE > 2 && tid == 0 && c + NSTAGE - 1 < nchunks) {
-                const int cn = c + NSTAGE - 1, sn = cn % NSTAGE;
-                fence_proxy_async();
-                mbar_expect_tx(&bars[sn], (uint32_t)Gm::stage_bytes(sizeof(T)));
-                tma_load_3d(s_in + (size_t)sn * IN_ROWS * SW, &tmap, &bars[sn], c_in0, r_in0 + cn * IN_ROWS, b);
-            }
             mbar_wait(&bars[stage], (uint32_t)((c / NSTAGE) & 1));
             // border CTAs: replace the zero-filled out-of-range halo by the boundary extension.
             // Only the samples some output of this strip / segment really reads are patched:
@@ -332,7 +322,7 @@ fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_consta
         }
         __syncthreads();   // ring rows of this chunk visible; the input stage is free again
 
-        if (USE_TMA && NSTAGE == 2 && tid == 0 && c + NSTAGE < nchunks) {
+        if (USE_TMA && tid == 0 && c + NSTAGE < nchunks) {
             fence_proxy_async();   // generic-proxy accesses to this stage precede the async refill
             mbar_expect_tx(&bars[stage], (uint32_t)Gm::stage_bytes(sizeof(T)));
             tma_load_3d(tile, &tmap, &bars[stage], c_in0, r_in0 + (c + NSTAGE) * IN_ROWS, b);
@@ -423,15 +413,15 @@ fwd2d_strip_kernel(const __grid_constant__ Fwd2dParams<T> p, const __grid_consta
 // ------------------------------------------------------------------------------------------
 template <int L, int TW>
 struct Fwd2dGeomF {
-    using Base = Fwd2dGeom<L, TW, 4, 2>;
+    using Base = Fwd2dGeom<L, TW, 4>;
     static constexpr int MIR = L + 2;
     static constexpr size_t SMEM = 2 * Base::stage_bytes(4) + 2 * (size_t)(Base::RING + MIR) * Base::MP * 4 + 64;
 };
 
 template <int L, int TW, bool USE_TMA>
-__global__ void __launch_bounds__((Fwd2dGeom<L, TW, 4, 2>::NTHREADS), 3)
+__global__ void __launch_bounds__((Fwd2dGeom<L, TW, 4>::NTHREADS), 3)
 fwd2d_strip_f32_kernel(const __grid_constant__ Fwd2dParams<float> p, const __grid_constant__ CUtensorMap tmap) {
-    using Gm = Fwd2dGeom<L, TW, 4, 2>;
+    using Gm = Fwd2dGeom<L, TW, 4>;
     constexpr int OFF = Gm::OFF, HAL = Gm::HAL, HALO = Gm::HALO, CH = Gm::CH, IN_ROWS = Gm::IN_ROWS, SW = Gm::SW;
     constexpr int MP = Gm::MP, RING = Gm::RING, NT = Gm::NTHREADS, NV4 = Gm::NV4, MIR = Fwd2dGeomF<L, TW>::MIR;
     constexpr int NCG = TW / 4;
@@ -637,11 +627,11 @@ static bool make_tmap_3d(CUtensorMap* map, const T* base, int64_t B, int64_t H, 
     return r == CUDA_SUCCESS;
 }
 
-template <typename T, int L, int TW, int NSTG = 2>
+template <typename T, int L, int TW>
 static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, T* const out[4],
                                       const int64_t out_bs[4], const int64_t out_rs[4], int Mh, int Mw, int mode,
                                       const Taps<T>& taps, cudaStream_t st, uint64_t* launches) {
-    using Gm = Fwd2dGeom<L, TW, sizeof(T), NSTG>;
+    using Gm = Fwd2dGeom<L, TW, sizeof(T)>;
     Fwd2dParams<T> p;
     p.x = x; p.x_bs = x_bs; p.x_rs = x_rs;
     for (int k = 0; k < 4; ++k) { p.out[k] = out[k]; p.out_bs[k] = out_bs[k]; p.out_rs[k] = out_rs[k]; }
@@ -669,8 +659,8 @@ static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64
     memset(&tmap, 0, sizeof(tmap));
     const bool tma = make_tmap_3d<T>(&tmap, x, B, H, W, x_bs, x_rs, Gm::SW, Gm::IN_ROWS);
     size_t smem = Gm::smem_bytes(sizeof(T));
-    auto kern = tma ? fwd2d_strip_kernel<T, L, TW, true, NSTG> : fwd2d_strip_kernel<T, L, TW, false, NSTG>;
-    if constexpr (sizeof(T) == 4 && TW == 64 && NSTG == 2) {
+    auto kern = tma ? fwd2d_strip_kernel<T, L, TW, true> : fwd2d_strip_kernel<T, L, TW, false>;
+    if constexpr (sizeof(T) == 4 && TW == 64) {
         if (!knob_on(K_NO_FFMA2)) {
             for (int m = 0; m < L / 2; ++m) {
                 p.pl[m] = make_float2(taps.lo[L - 1 - 2 * m], taps.lo[L - 2 - 2 * m]);
@@ -697,32 +687,6 @@ static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
-}
-
-template <int L>
-static cudaError_t launch_fwd2d_pair(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs,
-                                     const wt_level& l1, const wt_level& l2, int mode, const Taps<float>& taps,
-                                     cudaStream_t st, uint64_t* launches);
-static bool pair2d_supported(int L, int mode);
-
-template <typename T>
-static bool try_pair(const T*, int64_t, int, int, int64_t, int64_t, const wt_level&, const wt_level&, int, int,
-                     const Taps<T>&, cudaStream_t, uint64_t*, cudaError_t*) {
-    return false;
-}
-template <>
-bool try_pair<float>(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
-                     const wt_level& l2, int L, int mode, const Taps<float>& taps, cudaStream_t st,
-                     uint64_t* launches, cudaError_t* err) {
-    if (!pair2d_supported(L, mode)) return false;
-    if (l1.strides[1] != 1 || l2.strides[1] != 1 || l2.approx_strides[1] != 1) return false;
-    switch (L) {
-        case 2: *err = launch_fwd2d_pair<2>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches); return true;
-        case 4: *err = launch_fwd2d_pair<4>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches); return true;
-        case 6: *err = launch_fwd2d_pair<6>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches); return true;
-        case 8: *err = launch_fwd2d_pair<8>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches); return true;
-        default: return false;
-    }
 }
 
 template <typename T>
@@ -778,17 +742,12 @@ static int fused2d_fwd_try(int ndim, int mode, int levels, int L, const double* 
     // stream, so that the latency-bound deep levels of one chunk run under the bandwidth-bound level-1 launch
     // of the next.  The intermediate approximations cA_1 .. cA_{n-1} are scratch, so every chunk reuses the
     // scratch slots of its stream.  (Small chunks could keep those slots L2-resident, but with one launch per
-    // level and chunk the launch tails grow with the chunk count; the persistent kernel in fused2d_mega.cuh is
-    // the way to try that effect.)
+    // level and chunk the launch tails grow with the chunk count.)
     int64_t chunk = 0;   // images per chunk
     int nstreams = 2;
     if (knob_is_set(K_CHUNK)) chunk = knob_val(K_CHUNK, 0);
     else if (levels >= 2 && batch >= 16 && (int64_t)batch * dims[0] * dims[1] >= (int64_t(1) << 27)) chunk = (batch + 1) / 2;
     if (knob_is_set(K_STREAMS)) nstreams = knob_val(K_STREAMS, 2) >= 2 ? 2 : 1;
-    if (knob_is_set(K_SPLIT)) {   // legacy knob: number of equal chunks, no scratch reuse change
-        const int ns = (int)knob_val(K_SPLIT, 0);
-        chunk = ns > 1 ? (batch + ns - 1) / ns : 0;
-    }
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     if (nstreams > 1 && (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone)) nstreams = 1;
     if (knob_on(K_NO_AUX_STREAM)) nstreams = 1;
@@ -852,7 +811,6 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
     int64_t sbs = xbs, srs = xs[0];
     int64_t H = dims[0], W = dims[1];
     uint64_t launches = 0;
-    const int variant = (int)knob_val(K_FWD2D_VARIANT, 0);
     for (int l = 0; l < levels; ++l) {
         const wt_level& d = lv[l];
         if (H >= (1 << 30) || W >= (1 << 30)) break;
@@ -863,21 +821,6 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
                 g_launches.fetch_add(launches, std::memory_order_relaxed);
                 launches = 0;
                 if (pe != cudaSuccess) return cuda_fail(pe, "fwd2d_wpair_kernel");
-                const wt_level& d2 = lv[l + 1];
-                src = (const T*)d2.approx; sbs = d2.approx_batch_stride; srs = d2.approx_strides[0];
-                H = d2.dims[0]; W = d2.dims[1];
-                ++l;
-                *first_generic = l + 1;
-                continue;
-            }
-        }
-        if (l + 1 < levels) {
-            // two levels in one launch: the level-(l+1) approximation never leaves the SM
-            cudaError_t pe = cudaSuccess;
-            if (try_pair<T>(src, batch, (int)H, (int)W, sbs, srs, lv[l], lv[l + 1], L, mode, taps, st, &launches, &pe)) {
-                g_launches.fetch_add(launches, std::memory_order_relaxed);
-                launches = 0;
-                if (pe != cudaSuccess) return cuda_fail(pe, "fwd2d_pair_kernel");
                 const wt_level& d2 = lv[l + 1];
                 src = (const T*)d2.approx; sbs = d2.approx_batch_stride; srs = d2.approx_strides[0];
                 H = d2.dims[0]; W = d2.dims[1];
@@ -898,15 +841,8 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
         cudaError_t e = cudaSuccess;
 #define WTB_F2D_CASE(LL)                                                                                       \
     case LL:                                                                                                   \
-        if (variant == 1)                                                                                      \
-            e = launch_fwd2d_level<T, LL, (sizeof(T) == 4 ? 64 : 32), 3>(src, batch, (int)H, (int)W, sbs, srs, out, obs, ors, \
-                                                                         Mh, Mw, mode, taps, st, &launches);   \
-        else if (variant == 2)                                                                                 \
-            e = launch_fwd2d_level<T, LL, 32, 2>(src, batch, (int)H, (int)W, sbs, srs, out, obs, ors,             \
-                                                 Mh, Mw, mode, taps, st, &launches);                           \
-        else                                                                                                   \
-            e = launch_fwd2d_level<T, LL, (sizeof(T) == 4 ? 64 : 32), 2>(src, batch, (int)H, (int)W, sbs, srs, out, obs, ors, \
-                                                                         Mh, Mw, mode, taps, st, &launches);   \
+        e = launch_fwd2d_level<T, LL, (sizeof(T) == 4 ? 64 : 32)>(src, batch, (int)H, (int)W, sbs, srs, out, obs, ors, \
+                                                                  Mh, Mw, mode, taps, st, &launches);          \
         break;
         switch (L) {
             WTB_F2D_CASE(2)

@@ -19,9 +19,9 @@ namespace wtb {
 //   MATI_ROWS        > 0 row-streaming synthesis kernel with at most that many rows per CTA, < 0 exactly, 0 off
 //   MATI_MINCTAS, MATI_MERGE_N   short rows: halve the chunk below this CTA count / merge levels of rows <= N
 #define WTB_KNOB_LIST(X)                                                                                     \
-    X(DISABLE_FUSED) X(NO_FFMA2) X(CHUNK) X(STREAMS) X(SPLIT) X(FWD2D_VARIANT) X(MEGA) X(MEGA_SEG) X(MEGA_RING) \
-    X(MEGA_NOHINTS) X(ENABLE_PAIR) X(PAIR_TW2) X(FWD3D_TILE) X(CONVF_CHUNK) X(CONVF_K) X(MATF_CHUNK) X(MATI_CHUNK) \
-    X(MATF_K) X(MATI_K) X(MATI_NT) X(MATI_ROWS) X(MATI_MINCTAS) X(MATI_MERGE_N) X(MATF_MINCTAS) X(MATF_KCOARSE) X(NO_WPAIR) X(WPAIR_SEG) X(WPAIR_MIN) X(WPAIR_DEEP) X(MATF_VARIANT) X(FWD3D_VARIANT)    \
+    X(DISABLE_FUSED) X(NO_FFMA2) X(CHUNK) X(STREAMS) X(FWD3D_TILE) X(CONVF_CHUNK) X(CONVF_K) X(MATF_CHUNK)     \
+    X(MATI_CHUNK) X(MATF_K) X(MATI_K) X(MATI_NT) X(MATI_ROWS) X(MATI_MINCTAS) X(MATI_MERGE_N) X(MATF_MINCTAS)      \
+    X(MATF_KCOARSE) X(NO_WPAIR) X(WPAIR_SEG) X(WPAIR_MIN) X(WPAIR_DEEP) X(MATF_VARIANT)                            \
     X(NO_AUX_STREAM) X(WPAIR_VAR) X(WPAIR) X(MATF_NT) X(MATF_MINB) X(MATF_CPC) X(NO_DMMA) X(DMMA_PERM)
 
 enum KnobId {

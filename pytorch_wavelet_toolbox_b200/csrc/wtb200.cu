@@ -20,9 +20,6 @@
 #include "matrix_dmma.cuh"
 #include "axis1d_fused.cuh"
 #include "tap_grad.cuh"
-#if !defined(WTB_NO_FUSED) && !__has_include("fused2d.cuh")
-#define WTB_NO_FUSED 1
-#endif
 
 namespace wtb {
 
@@ -43,15 +40,11 @@ static int cuda_fail(cudaError_t e, const char* what) {
 }
 
 }  // namespace wtb
-#ifndef WTB_NO_FUSED
 #include "fused2d.cuh"
-#include "fused2d_pair.cuh"
 #include "fused2d_wpair.cuh"
-#include "fused2d_mega.cuh"
 #include "inv2d.cuh"
 #include "fwd3d.cuh"
 #include "inv3d.cuh"
-#endif
 namespace wtb {
 
 static inline int pad_left(int L) { return (2 * L - 3) / 2; }
@@ -451,22 +444,10 @@ static int dwt_fwd_t(int ndim, int mode, int levels, int L, const double* dlo, c
     int64_t s1, s2;
     generic_scratch_elems(ndim, L, levels, batch, dims, 0, &s1, &s2);
     int first_generic = 0;
-#ifndef WTB_NO_FUSED
     if constexpr (sizeof(T) == 4) {
         if (fused3d_fwd_covers(ndim, 4, L)) {
             int done = 0;
             int rc = fused3d_fwd_try(mode, levels, L, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, st, &done);
-            if (rc != 0 || done) return rc;
-        }
-        if (ndim == 2 && mega2d_enabled() && fused2d_fwd_covers(ndim, L) && xs[1] == 1) {
-            int done = 0, rc = 0;
-            switch (L) {
-                case 2: rc = launch_fwd2d_mega<2>(mode, levels, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, ws, ws_bytes, st, &done); break;
-                case 4: rc = launch_fwd2d_mega<4>(mode, levels, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, ws, ws_bytes, st, &done); break;
-                case 6: rc = launch_fwd2d_mega<6>(mode, levels, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, ws, ws_bytes, st, &done); break;
-                case 8: rc = launch_fwd2d_mega<8>(mode, levels, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, ws, ws_bytes, st, &done); break;
-                default: break;
-            }
             if (rc != 0 || done) return rc;
         }
     }
@@ -475,7 +456,6 @@ static int dwt_fwd_t(int ndim, int mode, int levels, int L, const double* dlo, c
                                     st, &first_generic);
         if (rc != 0) return rc;
     }
-#endif
     if (first_generic < levels) {
         if (ndim > 1 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
             return fail(WT_EWORKSPACE, "workspace: need %zu bytes, have %zu", (size_t)(s1 + s2) * sizeof(T), ws_bytes);
@@ -502,7 +482,6 @@ static int dwt_inv_t(int ndim, int levels, int L, const double* rlo, const doubl
         }
         if (!lv[l].details || !lv[l].approx) return fail(WT_EINVAL, "level %d: NULL buffer", l + 1);
     }
-#ifndef WTB_NO_FUSED
     if constexpr (sizeof(T) == 4) {
         if (fused2d_inv_covers(ndim, 4, L)) {
             int done = 0;
@@ -515,7 +494,6 @@ static int dwt_inv_t(int ndim, int levels, int L, const double* rlo, const doubl
             if (rc != 0 || done) return rc;
         }
     }
-#endif
     int64_t s1, s2;
     generic_scratch_elems(ndim, L, levels, batch, out_dims, 1, &s1, &s2);
     if (ndim > 1 && levels > 0 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
@@ -872,19 +850,16 @@ size_t wt_dwt_workspace_bytes(int ndim, int dtype, int levels, int filt_len, int
     if (ndim < 1 || ndim > 3 || !dims || levels <= 0) return 0;
     const bool general = (inverse & 2) != 0;   // bit 1: the requirement of the general path, whatever a fused path covers
     inverse &= 1;
-#ifndef WTB_NO_FUSED
     if (general) {
         // fall through to the general requirement
     } else if (!inverse && fused2d_fwd_covers(ndim, filt_len)) {
         // the fused path needs no scratch unless it has to bail out (odd strides); keep the
-        // general path's requirement only when the fused path is disabled.  The persistent multi-level
-        // kernel keeps its work-queue and completion counters in the workspace.
-        return (dtype == WT_F32 && mega2d_enabled()) ? mega_workspace_bytes(levels, batch) : 0;
+        // general path's requirement only when the fused path is disabled
+        return 0;
     }
     else if (inverse && fused2d_inv_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len)) return 0;
     else if (!inverse && fused3d_fwd_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len) && batch <= 65535) return 0;
     else if (inverse && fused3d_inv_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len) && batch <= 65535) return 0;
-#endif
     int64_t s1, s2;
     generic_scratch_elems(ndim, filt_len, levels, batch, dims, inverse, &s1, &s2);
     return (size_t)(s1 + s2) * (dtype == WT_F64 ? 8 : 4);

@@ -518,20 +518,6 @@ def test_host_pipeline_equals_device_path(monkeypatch):
         assert torch.equal(a, b.cpu())
 
 
-def test_pair_kernel_when_enabled(knob):
-    """The experimental two-level fused kernel (WTB200_ENABLE_PAIR=1) must agree with the oracle."""
-    knob("ENABLE_PAIR", 1)
-    knob("NO_WPAIR", 1)
-    g = torch.Generator().manual_seed(22)
-    for mode in ("zero", "constant", "reflect", "symmetric"):
-        for shape in ((300, 200), (129, 517), (64, 64)):
-            x = torch.randn((2,) + shape, generator=g)
-            _cmp_tree(wt.wavedec2(x.to(DEV), "db4", mode=mode, level=4 if min(shape) > 100 else 2),
-                      P.wavedec2(x, "db4", mode=mode, level=4 if min(shape) > 100 else 2), f"pair {mode} {shape}")
-            _cmp_tree(wt.wavedec2(x.to(DEV), "db2", mode=mode, level=3), P.wavedec2(x, "db2", mode=mode, level=3),
-                      f"pair db2 {mode} {shape}")
-
-
 def test_separable_front_ends():
     """fswavedec2/3 + fswaverec2/3 (SURVEY 8f row 1): dict containers over the fused kernels."""
     g = torch.Generator().manual_seed(23)
@@ -608,24 +594,6 @@ def test_tiny_and_ragged_shapes():
             _cmp_tree(wt.wavedec2(x.float().to(DEV), "db2", level=1, mode=mode), P.wavedec2(x.float(), "db2", level=1, mode=mode), f"tiny f32 {shape}")
     v = torch.randn(2, 5, 6, 70, generator=g)
     _cmp_tree(wt.wavedec3(v.to(DEV), "haar", level=1, mode="symmetric"), P.wavedec3(v, "haar", level=1, mode="symmetric"), "thin volume")
-
-
-@pytest.mark.parametrize("ring", ["0", "2", "3"])
-def test_persistent_multilevel_kernel_when_enabled(knob, ring):
-    """The experimental persistent all-levels kernel (WTB200_MEGA=1: work queue + completion counters +
-    TMA reads of data written by other SMs) must agree with the oracle, for every boundary mode."""
-    knob("MEGA", 1)
-    knob("MEGA_RING", int(ring))   # > 0: intermediate approximations in `ring` reused scratch slots
-    knob("MEGA_SEG", 64)
-    g = torch.Generator().manual_seed(61)
-    for mode in MODES:
-        for shape, lev in (((5, 300, 200), 3), ((3, 640, 520), 4), ((9, 64, 96), 2)):
-            x = torch.randn(shape, generator=g)
-            try:
-                want = P.wavedec2(x, "db4", mode=mode, level=lev)
-            except RuntimeError:
-                continue
-            _cmp_tree(wt.wavedec2(x.to(DEV), "db4", mode=mode, level=lev), want, f"mega {mode} {shape}")
 
 
 def test_calls_can_be_captured_in_a_cuda_graph():
