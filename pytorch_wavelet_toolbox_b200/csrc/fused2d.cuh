@@ -76,14 +76,14 @@ __device__ __forceinline__ float2 ffma2(const float2 a, const float2 b, const fl
     return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
-// Row filter of one thread: 8 consecutive (lo, hi) outputs from the register window v[].
+// Row filter of one thread: NG consecutive (lo, hi) outputs from the register window v[].
 // out[g] = sum_k dec[L-1-k] v[2g+k+OFF], evaluated as an even-tap and an odd-tap partial sum in the
 // two halves of one paired accumulator.
-template <int L, int OFF, int NV>
-__device__ __forceinline__ void row_filter8(const float (&v)[NV], const float2* __restrict__ pl,
-                                            const float2* __restrict__ ph, float (&lo)[8], float (&hi)[8]) {
+template <int L, int OFF, int NV, int NG>
+__device__ __forceinline__ void row_filter(const float (&v)[NV], const float2* __restrict__ pl,
+                                           const float2* __restrict__ ph, float (&lo)[NG], float (&hi)[NG]) {
 #pragma unroll
-    for (int g = 0; g < 8; ++g) {
+    for (int g = 0; g < NG; ++g) {
         float2 a = make_float2(0.f, 0.f), h = make_float2(0.f, 0.f);
 #pragma unroll
         for (int m = 0; m < L / 2; ++m) {
@@ -136,7 +136,7 @@ struct Fwd2dParams {
     int batch0;              // batch offset of this launch (gridDim.z chunking)
     int vec_store;           // 1: every output row start is 16-byte aligned -> 128-bit stores
     Taps<T> taps;            // un-flipped dec_lo / dec_hi
-    // float32 fast kernel: taps packed in pairs (see row_filter8 / col_filter2x4)
+    // float32 fast kernel: taps packed in pairs (see row_filter / col_filter2x4)
     float2 pl[8], ph[8], bl[16], bh[16];
 };
 
@@ -418,12 +418,79 @@ struct Fwd2dGeomF {
     static constexpr size_t SMEM = 2 * Base::stage_bytes(4) + 2 * (size_t)(Base::RING + MIR) * Base::MP * 4 + 64;
 };
 
+// Border CTAs of the TMA path: replace the zero-filled out-of-range halo of a staged float32 chunk by the
+// boundary extension.  Only the samples some needed output reads are patched: tile columns [0, nl) and
+// [cr0, cr1) of the in-range rows, and tile columns [0, cr1) of the out-of-range rows [0, nt) and [rb0, rb1).
+// Ends with a barrier when it wrote anything.
+template <int SW, int IN_ROWS, int NT>
+__device__ __forceinline__ void patch_tile_f32(float* tile, const float* __restrict__ xb, int64_t x_rs, int H, int W,
+                                               int mode, int c_in0, int r_base, int c_need1, int r_need1, int tid) {
+    const int nl = c_in0 < 0 ? -c_in0 : 0;
+    const int cr1 = min(c_need1 - c_in0, SW);
+    const int cr0 = max(min(W - c_in0, cr1), nl);
+    const int nt = r_base < 0 ? min(-r_base, IN_ROWS) : 0;
+    const int rb1 = min(r_need1 - r_base, IN_ROWS);
+    const int rb0 = max(min(H - r_base, rb1), nt);
+    const int wb = nl + (cr1 - cr0);
+    const bool patch = (wb > 0) || (nt > 0) || (rb1 > rb0);
+    if (!patch) return;
+    const int n_in = rb0 - nt;
+    for (int idx = tid; idx < n_in * wb; idx += NT) {
+        const int rr = nt + idx / wb, q = idx % wb;
+        const int cc = q < nl ? q : cr0 + (q - nl);
+        const int sc = ext_index32(c_in0 + cc, W, mode);
+        tile[rr * SW + cc] = __ldg(xb + (int64_t)(r_base + rr) * x_rs + sc);
+    }
+    const int n_oob = nt + (rb1 - rb0);
+    if (n_oob > 0 && cr1 > 0) {
+        for (int idx = tid; idx < n_oob * cr1; idx += NT) {
+            const int q = idx / cr1, cc = idx % cr1;
+            const int rr = q < nt ? q : rb0 + (q - nt);
+            const int sr = ext_index32(r_base + rr, H, mode);
+            const int sc = ext_index32(c_in0 + cc, W, mode);
+            tile[rr * SW + cc] = __ldg(xb + (int64_t)sr * x_rs + sc);
+        }
+    }
+    __syncthreads();
+}
+
+// Row pass of the float32 strip kernels: lane <-> tile row, warp <-> 8 output columns; writes the lo / hi lines
+// of the chunk into the ring (and into the mirror rows behind it).
+template <int L, int TW>
+__device__ __forceinline__ void strip_row_pass_f32(const float* tile, float* s_lo, float* s_hi, int ring_base,
+                                                   const float2* __restrict__ pl, const float2* __restrict__ ph,
+                                                   int lane, int warp) {
+    using Gm = Fwd2dGeom<L, TW, 4>;
+    constexpr int SW = Gm::SW, MP = Gm::MP, RING = Gm::RING, NV4 = Gm::NV4, MIR = L + 2;
+    const float* src = tile + lane * SW + 16 * warp;
+    float v[4 * NV4];
+#pragma unroll
+    for (int q = 0; q < NV4; ++q) {
+        const float4 t = *reinterpret_cast<const float4*>(src + 4 * q);
+        v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+    }
+    float lo[8], hi[8];
+    row_filter<L, Gm::OFF>(v, pl, ph, lo, hi);
+    int slot = ring_base + lane;
+    if (slot >= RING) slot -= RING;
+    float* dlo = s_lo + slot * MP + 8 * warp;
+    float* dhi = s_hi + slot * MP + 8 * warp;
+    const float4 l0 = make_float4(lo[0], lo[1], lo[2], lo[3]), l1 = make_float4(lo[4], lo[5], lo[6], lo[7]);
+    const float4 h0 = make_float4(hi[0], hi[1], hi[2], hi[3]), h1 = make_float4(hi[4], hi[5], hi[6], hi[7]);
+    *reinterpret_cast<float4*>(dlo) = l0; *reinterpret_cast<float4*>(dlo + 4) = l1;
+    *reinterpret_cast<float4*>(dhi) = h0; *reinterpret_cast<float4*>(dhi + 4) = h1;
+    if (slot < MIR) {
+        *reinterpret_cast<float4*>(dlo + RING * MP) = l0; *reinterpret_cast<float4*>(dlo + RING * MP + 4) = l1;
+        *reinterpret_cast<float4*>(dhi + RING * MP) = h0; *reinterpret_cast<float4*>(dhi + RING * MP + 4) = h1;
+    }
+}
+
 template <int L, int TW, bool USE_TMA>
 __global__ void __launch_bounds__((Fwd2dGeom<L, TW, 4>::NTHREADS), 3)
 fwd2d_strip_f32_kernel(const __grid_constant__ Fwd2dParams<float> p, const __grid_constant__ CUtensorMap tmap) {
     using Gm = Fwd2dGeom<L, TW, 4>;
-    constexpr int OFF = Gm::OFF, HAL = Gm::HAL, HALO = Gm::HALO, CH = Gm::CH, IN_ROWS = Gm::IN_ROWS, SW = Gm::SW;
-    constexpr int MP = Gm::MP, RING = Gm::RING, NT = Gm::NTHREADS, NV4 = Gm::NV4, MIR = Fwd2dGeomF<L, TW>::MIR;
+    constexpr int HAL = Gm::HAL, HALO = Gm::HALO, CH = Gm::CH, IN_ROWS = Gm::IN_ROWS, SW = Gm::SW;
+    constexpr int MP = Gm::MP, RING = Gm::RING, NT = Gm::NTHREADS, MIR = Fwd2dGeomF<L, TW>::MIR;
     constexpr int NCG = TW / 4;
     static_assert(NT == 2 * (CH / 2) * NCG, "one column-pass item per thread");
 
@@ -484,36 +551,8 @@ fwd2d_strip_f32_kernel(const __grid_constant__ Fwd2dParams<float> p, const __gri
 
         if (USE_TMA) {
             mbar_wait(&bars[stage], (uint32_t)((c >> 1) & 1));
-            if (p.mode != WT_MODE_ZERO) {
-                const int nl = c_in0 < 0 ? -c_in0 : 0;
-                const int cr1 = min(c_need1 - c_in0, SW);
-                const int cr0 = max(min(p.W - c_in0, cr1), nl);
-                const int nt = r_base < 0 ? min(-r_base, IN_ROWS) : 0;
-                const int rb1 = min(r_need1 - r_base, IN_ROWS);
-                const int rb0 = max(min(p.H - r_base, rb1), nt);
-                const int wb = nl + (cr1 - cr0);
-                const bool patch = (wb > 0) || (nt > 0) || (rb1 > rb0);
-                if (patch) {
-                    const int n_in = rb0 - nt;
-                    for (int idx = tid; idx < n_in * wb; idx += NT) {
-                        const int rr = nt + idx / wb, q = idx % wb;
-                        const int cc = q < nl ? q : cr0 + (q - nl);
-                        const int sc = ext_index32(c_in0 + cc, p.W, p.mode);
-                        tile[rr * SW + cc] = __ldg(xb + (int64_t)(r_base + rr) * p.x_rs + sc);
-                    }
-                    const int n_oob = nt + (rb1 - rb0);
-                    if (n_oob > 0 && cr1 > 0) {
-                        for (int idx = tid; idx < n_oob * cr1; idx += NT) {
-                            const int q = idx / cr1, cc = idx % cr1;
-                            const int rr = q < nt ? q : rb0 + (q - nt);
-                            const int sr = ext_index32(r_base + rr, p.H, p.mode);
-                            const int sc = ext_index32(c_in0 + cc, p.W, p.mode);
-                            tile[rr * SW + cc] = __ldg(xb + (int64_t)sr * p.x_rs + sc);
-                        }
-                    }
-                    __syncthreads();
-                }
-            }
+            if (p.mode != WT_MODE_ZERO)
+                patch_tile_f32<SW, IN_ROWS, NT>(tile, xb, p.x_rs, p.H, p.W, p.mode, c_in0, r_base, c_need1, r_need1, tid);
         } else {
             for (int idx = tid; idx < IN_ROWS * SW; idx += NT) {
                 const int rr = idx / SW, cc = idx - rr * SW;
@@ -523,30 +562,7 @@ fwd2d_strip_f32_kernel(const __grid_constant__ Fwd2dParams<float> p, const __gri
             __syncthreads();
         }
 
-        // ---- row pass ---------------------------------------------------------------------------
-        {
-            const float* src = tile + lane * SW + 16 * warp;
-            float v[4 * NV4];
-#pragma unroll
-            for (int q = 0; q < NV4; ++q) {
-                const float4 t = *reinterpret_cast<const float4*>(src + 4 * q);
-                v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
-            }
-            float lo[8], hi[8];
-            row_filter8<L, OFF>(v, p.pl, p.ph, lo, hi);
-            int slot = ring_base + lane;
-            if (slot >= RING) slot -= RING;
-            float* dlo = s_lo + slot * MP + 8 * warp;
-            float* dhi = s_hi + slot * MP + 8 * warp;
-            const float4 l0 = make_float4(lo[0], lo[1], lo[2], lo[3]), l1 = make_float4(lo[4], lo[5], lo[6], lo[7]);
-            const float4 h0 = make_float4(hi[0], hi[1], hi[2], hi[3]), h1 = make_float4(hi[4], hi[5], hi[6], hi[7]);
-            *reinterpret_cast<float4*>(dlo) = l0; *reinterpret_cast<float4*>(dlo + 4) = l1;
-            *reinterpret_cast<float4*>(dhi) = h0; *reinterpret_cast<float4*>(dhi + 4) = h1;
-            if (slot < MIR) {
-                *reinterpret_cast<float4*>(dlo + RING * MP) = l0; *reinterpret_cast<float4*>(dlo + RING * MP + 4) = l1;
-                *reinterpret_cast<float4*>(dhi + RING * MP) = h0; *reinterpret_cast<float4*>(dhi + RING * MP + 4) = h1;
-            }
-        }
+        strip_row_pass_f32<L, TW>(tile, s_lo, s_hi, ring_base, p.pl, p.ph, lane, warp);
         __syncthreads();
 
         if (USE_TMA && tid == 0 && c + 2 < nchunks) {
@@ -692,6 +708,9 @@ static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64
 template <typename T>
 static bool try_wpair(const T*, int64_t, int, int, int64_t, int64_t, const wt_level&, const wt_level&, int, int,
                       const Taps<T>&, cudaStream_t, uint64_t*, cudaError_t*);
+template <typename T>
+static bool try_fuse2(const T*, int64_t, int, int, int64_t, int64_t, const wt_level&, const wt_level&, int, int,
+                      const Taps<T>&, cudaStream_t, uint64_t*, cudaError_t*);
 
 static bool fused2d_fwd_covers(int ndim, int L) {
     return ndim == 2 && !(L & 1) && L <= 16 && !knob_on(K_DISABLE_FUSED);
@@ -814,13 +833,22 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
     for (int l = 0; l < levels; ++l) {
         const wt_level& d = lv[l];
         if (H >= (1 << 30) || W >= (1 << 30)) break;
-        if (l + 1 < levels && (int64_t)batch * H * W >= knob_val(K_WPAIR_MIN, int64_t(1) << 24) && (l == 0 || knob_on(K_WPAIR_DEEP))) {
-            // two levels in one launch of independent warps (fused2d_wpair.cuh): cA_{l+1} stays in shared memory
+        if (l + 1 < levels) {
+            // two levels in one launch, cA_{l+1} stays in shared memory: the kernel of independent warps
+            // (fused2d_wpair.cuh) for levels 1-2 of images of >= WPAIR_MIN samples, at least 8 of them, else the
+            // opt-in two-level strip kernel (fused2d_fuse2.cuh)
             cudaError_t pe = cudaSuccess;
-            if (try_wpair<T>(src, batch, (int)H, (int)W, sbs, srs, lv[l], lv[l + 1], L, mode, taps, st, &launches, &pe)) {
+            const char* pair = nullptr;
+            const int64_t wmin = knob_val(K_WPAIR_MIN, int64_t(1) << 24);
+            if (H * W >= wmin && batch * H * W >= 8 * wmin && (l == 0 || knob_on(K_WPAIR_DEEP)) &&
+                try_wpair<T>(src, batch, (int)H, (int)W, sbs, srs, lv[l], lv[l + 1], L, mode, taps, st, &launches, &pe))
+                pair = "fwd2d_wpair_kernel";
+            else if (try_fuse2<T>(src, batch, (int)H, (int)W, sbs, srs, lv[l], lv[l + 1], L, mode, taps, st, &launches, &pe))
+                pair = "fwd2d_fuse2_f32_kernel";
+            if (pair) {
                 g_launches.fetch_add(launches, std::memory_order_relaxed);
                 launches = 0;
-                if (pe != cudaSuccess) return cuda_fail(pe, "fwd2d_wpair_kernel");
+                if (pe != cudaSuccess) return cuda_fail(pe, pair);
                 const wt_level& d2 = lv[l + 1];
                 src = (const T*)d2.approx; sbs = d2.approx_batch_stride; srs = d2.approx_strides[0];
                 H = d2.dims[0]; W = d2.dims[1];

@@ -78,7 +78,7 @@ struct WPairGeom {
     static_assert(RING >= L, "ring too small for the window of one output row");
 };
 
-// lo[c], hi[c] for NC consecutive outputs from the register window w (see row_filter8)
+// lo[c], hi[c] for NC consecutive outputs from the register window w (see row_filter)
 template <int L, int NC, int OFF, int NW>
 __device__ __forceinline__ void wp_rowfilt(const float (&w)[NW], const float2* __restrict__ pl,
                                            const float2* __restrict__ ph, float (&lo)[NC], float (&hi)[NC]) {
@@ -522,9 +522,13 @@ template <>
 bool try_wpair<float>(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
                       const wt_level& l2, int L, int mode, const Taps<float>& taps, cudaStream_t st,
                       uint64_t* launches, cudaError_t* err) {
-    // Opt-in (WTB200_WPAIR=1 / wt_set_knob("WPAIR", 1)): parity green and less DRAM traffic than one launch per
-    // level (cA1 never reaches HBM), but bound by instruction issue rather than by bytes, so it is not the default.
-    if (!knob_on(K_WPAIR) || knob_on(K_NO_WPAIR) || knob_on(K_DISABLE_FUSED)) return false;
+    // Default for levels (1, 2) of batches of >= 8 images of >= WPAIR_MIN = 2^24 samples (the caller checks): cA1
+    // never reaches HBM.  On an H100 80GB HBM3 at a 400 W power limit (tools/time_fwd2d_pairs.py), db4 level 4 takes
+    // 4.64 ms against 5.67 ms with one strip-kernel launch per level for 64 x 4096^2 and 0.68 against 0.76 ms for
+    // 8 x 4096^2; one 4096^2 image (0.25 against 0.17 ms) and images of 2048^2 and smaller (up to 40 % slower) are
+    // faster with one launch per level.  WPAIR=0 or NO_WPAIR=1 (environment
+    // WTB200_<NAME> or wt_set_knob) forces one launch per level.
+    if ((knob_is_set(K_WPAIR) && !knob_on(K_WPAIR)) || knob_on(K_NO_WPAIR) || knob_on(K_DISABLE_FUSED)) return false;
     switch (L) {
         case 2: return launch_fwd2d_wpair_t<2, 3, 12>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches, err);
         case 4: return launch_fwd2d_wpair_t<4, 3, 12>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, st, launches, err);

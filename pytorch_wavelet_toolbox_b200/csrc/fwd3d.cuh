@@ -197,7 +197,7 @@ fwd3d_tile_kernel(const __grid_constant__ Fwd3dParams p, const __grid_constant__
                 v[4 * qd] = f.x; v[4 * qd + 1] = f.y; v[4 * qd + 2] = f.z; v[4 * qd + 3] = f.w;
             }
             float lo[8], hi[8];
-            row_filter8<L, OFF>(v, p.pl, p.ph, lo, hi);
+            row_filter<L, OFF>(v, p.pl, p.ph, lo, hi);
             float* dlo = s_lo + row * MP + 8 * grp;
             float* dhi = s_hi + row * MP + 8 * grp;
             *reinterpret_cast<float4*>(dlo) = make_float4(lo[0], lo[1], lo[2], lo[3]);

@@ -22,7 +22,7 @@ namespace wtb {
     X(DISABLE_FUSED) X(NO_FFMA2) X(CHUNK) X(STREAMS) X(FWD3D_TILE) X(CONVF_CHUNK) X(CONVF_K) X(MATF_CHUNK)     \
     X(MATI_CHUNK) X(MATF_K) X(MATI_K) X(MATI_NT) X(MATI_ROWS) X(MATI_MINCTAS) X(MATI_MERGE_N) X(MATF_MINCTAS)      \
     X(MATF_KCOARSE) X(NO_WPAIR) X(WPAIR_SEG) X(WPAIR_MIN) X(WPAIR_DEEP) X(MATF_VARIANT)                            \
-    X(NO_AUX_STREAM) X(WPAIR_VAR) X(WPAIR) X(MATF_NT) X(MATF_MINB) X(MATF_CPC) X(NO_DMMA) X(DMMA_PERM)
+    X(NO_AUX_STREAM) X(WPAIR_VAR) X(WPAIR) X(MATF_NT) X(MATF_MINB) X(MATF_CPC) X(NO_DMMA) X(DMMA_PERM) X(FUSE2)
 
 enum KnobId {
 #define X(n) K_##n,

@@ -42,6 +42,7 @@ static int cuda_fail(cudaError_t e, const char* what) {
 }  // namespace wtb
 #include "fused2d.cuh"
 #include "fused2d_wpair.cuh"
+#include "fused2d_fuse2.cuh"
 #include "inv2d.cuh"
 #include "fwd3d.cuh"
 #include "inv3d.cuh"
