@@ -240,7 +240,7 @@ void wt_launch_count_reset(void);
 /* Tuning / test switches (NOT part of the drop-in surface).  Every switch is also read ONCE from the
  * environment variable WTB200_<NAME> when the library is first used; no transform call reads the environment.
  * Names: DISABLE_FUSED (general kernels only), NO_WPAIR (one launch per 2-D analysis level), WPAIR_SEG,
- * WPAIR_MIN, WPAIR_DEEP, FUSE2 (opt-in two-level 2-D strip kernel), CHUNK, STREAMS, NO_AUX_STREAM, NO_DMMA, MATF_VARIANT, ... (csrc/knobs.cuh).
+ * WPAIR_MIN, WPAIR_DEEP, FUSE2 (opt-in two-level 2-D strip kernel), CHUNK, STREAMS, NO_AUX_STREAM, NO_DMMA, MATF_K, MATI_K, ... (csrc/knobs.cuh).
  * wt_set_knob returns 0 or WT_EINVAL for an unknown name; wt_get_knob returns 1 and the value when the switch
  * is set, 0 when it is not, WT_EINVAL for an unknown name. */
 int wt_set_knob(const char* name, long long value);

@@ -11,18 +11,16 @@
 namespace wtb {
 
 // Matrix FWT (matrix_dmma.cuh, matrix_fused.cuh):
-//   NO_DMMA          float64 without the FP64 tensor-core cascades (scalar fused / per-level kernels)
-//   MATF_VARIANT     1 = streaming DMMA analysis kernel instead of the polyphase one
-//   MATF_K / MATI_K  levels per launch (analysis / synthesis);  MATF_KCOARSE the same for rows <= 8192 samples
+//   NO_DMMA          float64 without the FP64 tensor-core cascades (scalar fused analysis, per-level synthesis)
+//   MATF_K / MATI_K  levels per launch (analysis / float64 synthesis);  MATF_KCOARSE the same for rows <= 8192 samples
 //   MATF_CHUNK / MATI_CHUNK   finest-level samples per CTA;  MATF_NT / MATI_NT  threads per CTA (128 | 256)
-//   MATF_CPC, MATF_MINCTAS    streaming kernels: chunks per CTA and the CTA count it is lowered for
-//   MATI_ROWS        > 0 row-streaming synthesis kernel with at most that many rows per CTA, < 0 exactly, 0 off
+//   MATF_CPC         scalar fused analysis: consecutive chunks one CTA streams
 //   MATI_MINCTAS, MATI_MERGE_N   short rows: halve the chunk below this CTA count / merge levels of rows <= N
 #define WTB_KNOB_LIST(X)                                                                                     \
     X(DISABLE_FUSED) X(NO_FFMA2) X(CHUNK) X(STREAMS) X(FWD3D_TILE) X(CONVF_CHUNK) X(CONVF_K) X(MATF_CHUNK)     \
-    X(MATI_CHUNK) X(MATF_K) X(MATI_K) X(MATI_NT) X(MATI_ROWS) X(MATI_MINCTAS) X(MATI_MERGE_N) X(MATF_MINCTAS)      \
-    X(MATF_KCOARSE) X(NO_WPAIR) X(WPAIR_SEG) X(WPAIR_MIN) X(WPAIR_DEEP) X(MATF_VARIANT)                            \
-    X(NO_AUX_STREAM) X(WPAIR_VAR) X(WPAIR) X(MATF_NT) X(MATF_MINB) X(MATF_CPC) X(NO_DMMA) X(DMMA_PERM) X(FUSE2)
+    X(MATI_CHUNK) X(MATF_K) X(MATI_K) X(MATI_NT) X(MATI_MINCTAS) X(MATI_MERGE_N)                               \
+    X(MATF_KCOARSE) X(NO_WPAIR) X(WPAIR_SEG) X(WPAIR_MIN) X(WPAIR_DEEP)                                            \
+    X(NO_AUX_STREAM) X(WPAIR_VAR) X(WPAIR) X(MATF_NT) X(MATF_MINB) X(MATF_CPC) X(NO_DMMA) X(FUSE2)
 
 enum KnobId {
 #define X(n) K_##n,

@@ -3,20 +3,18 @@
 // north_star: "tensor cores are used only for the MatrixWavedec path where the boundary-filter sparse matmul is
 // reformulated as a banded dense contraction".  The level operator A_n of the reference
 // (torch.sparse.mm(A_level, .), src/ptwt/matmul_transform.py:409-425) is block-Toeplitz away from its corner blocks:
-// every output pair (lo[i], hi[i]) is the same L-tap window sliding by two samples.  Four consecutive outputs of both
-// bands (8 rows) read one window of L + 6 samples, so a tile of 8 such groups is the dense product
+// every output pair (lo[i], hi[i]) is the same L-tap window sliding by two samples, and the synthesis operator has
+// the same structure.  So a tile of consecutive outputs is a small dense product of a window of the input (A operand)
+// and a matrix of filter taps (B operand, registers), evaluated with mma.sync.aligned.m8n8k4.f64 (DMMA, the FP64
+// tensor-core instruction of sm_90; wgmma has no f64 kind).  Part of the filter matrix is structural zeros -- the
+// price of the dense form.
 //
-//     D[8 x 8] = A[8 x (L+6)] * B[(L+6) x 8],   A[(band, s)][u] = f_band[u - 2 s],   B[u][g] = x[2 i0 + 8 g - HL + u]
-//
-// evaluated with mma.sync.aligned.m8n8k4.f64 (DMMA, the FP64 tensor-core instruction of sm_90; wgmma has no f64
-// kind): about (L+6)/4 instructions of 256 FMAs for 64 outputs.  60 % of those FMAs multiply structural zeros of A --
-// the price of the dense form -- but the scalar kernel is bound by instruction issue, not by the FP64 pipe, and the
-// DMMA form needs ~0.3 warp instructions per output instead of 1.5.
-//
-// Everything around the contraction is the streaming cascade of matrix_fused.cuh: a CTA takes consecutive chunks of one
-// row through K levels, level inputs live in shared memory (interleaved, as the B fragment wants them), the next chunk
-// arrives by cp.async meanwhile, details go to HBM, the corner blocks (dense orthogonalised boundary rows) are applied
-// by scalar code in the CTAs at the two ends.
+// Two kernels, each taking a group of levels through shared memory in one launch, so that only the details and the
+// last approximation of a group (analysis) or its finest output (synthesis) reach HBM:
+//   mat_fwd_dmma2_kernel  MatrixWavedec, the polyphase analysis cascade
+//   mat_inv_dmma_kernel   MatrixWaverec, the synthesis cascade
+// The corner blocks (dense orthogonalised boundary rows) are applied by scalar code in the CTAs at the two ends of a
+// row.
 #pragma once
 
 #include "matrix_fused.cuh"
@@ -29,282 +27,9 @@ __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, const double
                  : "d"(a), "d"(b));
 }
 
-template <int L, int NT, bool PERM>
-__global__ void __launch_bounds__(NT) mat_fwd_dmma_kernel(const __grid_constant__ MatFusedParams<double> p) {
-    constexpr int HL = L / 2 - 1, HR = L / 2;
-    // The contraction index u (window sample of a group of 4 outputs) is split as u = E * k + e: lane k of a fragment
-    // column holds E CONSECUTIVE samples (E even, window start shifted by SH to an even sample), so the B fragments of
-    // one tile are E / 2 aligned 128-bit shared loads per lane (conflict-free for E = 6) instead of one 64-bit load per
-    // k-step with 4-way bank conflicts; the A fragment is permuted the same way.
-    // PERM = false: u = 4 e + k (E = ceil((L + 6) / 4) k-steps, one 64-bit load each, 4-way conflicts).
-    constexpr int SH = PERM ? (HL & 1) : 0;
-    constexpr int E = PERM ? ((L + 6 + SH + 3) / 4 + 1) / 2 * 2 : (L + 6 + 3) / 4;
-    constexpr int KS = PERM ? E : 1;              // stride of the lane index k in the window
-    constexpr int ES = PERM ? 1 : 4;              // stride of the k-step e in the window
-    constexpr int NW = NT / 32;
-
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    double* raw0 = reinterpret_cast<double*>(smem_raw);   // level-0 samples of the current / next chunk (two buffers)
-    double* raw1 = raw0 + p.cap0;
-    double* levA = raw1 + p.cap0;                          // approximations, alternating
-    double* levB = levA + (p.cap0 / 2 + 16);
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int b = blockIdx.y;
-    const int K = p.k;
-    const double* __restrict__ xb = p.x + (int64_t)b * p.x_stride;
-
-    __shared__ int s_r[2][2][MATF_MAXK + 1];
-    const int nchunks = (p.n[K] + p.tk - 1) / p.tk;
-    const int c_first = blockIdx.x * p.cpc, c_last = min(c_first + p.cpc, nchunks);
-    if (c_first >= nchunks) return;
-    auto ranges = [&](int chunk, int set) {
-        int lo_j = chunk * p.tk, hi_j = min(lo_j + p.tk, p.n[K]);
-        s_r[set][0][K] = lo_j; s_r[set][1][K] = hi_j;
-        for (int j = K; j >= 1; --j) {
-            const int half = p.n[j];
-            int lo = 2 * lo_j - HL, hi = 2 * (hi_j - 1) + HR + 1;
-            if (lo_j < p.nb_top[j - 1]) lo = 0, hi = max(hi, p.w_left[j - 1]);
-            if (hi_j > half - p.nb_bot[j - 1]) hi = p.n[j - 1], lo = min(lo, p.n[j - 1] - p.w_right[j - 1]);
-            lo = max(lo, 0) & ~3;
-            hi = min(hi, p.n[j - 1]);
-            s_r[set][0][j - 1] = lo_j = lo;
-            s_r[set][1][j - 1] = hi_j = hi;
-        }
-    };
-    auto prefetch = [&](double* dst, int s0, int s1) {
-        const int cnt = s1 - s0, nv = cnt / 2;
-        for (int q = tid; q < nv; q += NT) {
-            const unsigned d = (unsigned)__cvta_generic_to_shared(dst + 2 * q);
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(xb + s0 + 2 * q) : "memory");
-        }
-        if ((cnt & 1) && tid == 0) {
-            const unsigned d = (unsigned)__cvta_generic_to_shared(dst + cnt - 1);
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(xb + s1 - 1) : "memory");
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-
-    // A fragment (row-major 8 x 4 per k-step e): this lane holds A[m = lane / 4][u = E * (lane % 4) + e],
-    // row m = 4 * band + s  ->  f_band[u - SH - 2 s]
-    double afrag[E];
-    {
-        const int m = lane >> 2, band = m >> 2, s = m & 3;
-#pragma unroll
-        for (int e = 0; e < E; ++e) {
-            const int kk = KS * (lane & 3) + ES * e - SH - 2 * s;
-            afrag[e] = (kk >= 0 && kk < L) ? (band ? p.fhi[kk] : p.flo[kk]) : 0.0;
-        }
-    }
-    const int frag_n = lane >> 2, frag_k = lane & 3;      // B fragment: B[k = lane % 4][n = lane / 4]
-    const int out_band = lane >> 4, out_s = (lane >> 2) & 3;
-    const int out_g0 = 2 * (lane & 3);                     // D fragment: columns (groups) 2 (lane % 4), + 1
-
-    if (tid == 0) ranges(c_first, 0);
-    __syncthreads();
-    prefetch(raw0, s_r[0][0][0], s_r[0][1][0]);
-
-    int set = 0;
-    for (int chunk = c_first; chunk < c_last; ++chunk, set ^= 1) {
-        const int* rlo = s_r[set][0];
-        const int* rhi = s_r[set][1];
-        double* in = set ? raw1 : raw0;
-        if (tid == 0 && chunk + 1 < c_last) ranges(chunk + 1, set ^ 1);
-        asm volatile("cp.async.wait_all;" ::: "memory");
-        __syncthreads();                              // this chunk's samples landed; the next chunk's ranges are visible
-        if (chunk + 1 < c_last) prefetch(set ? raw0 : raw1, s_r[set ^ 1][0][0], s_r[set ^ 1][1][0]);
-
-        double* nxt = levA;
-#pragma unroll 1
-        for (int j = 1; j <= K; ++j) {
-            const int half = p.n[j], nprev = p.n[j - 1];
-            const int in0 = rlo[j - 1], in_cnt = rhi[j - 1] - rlo[j - 1];
-            const int o0 = rlo[j], o1 = rhi[j];
-            const int own0 = (chunk * p.tk) << (K - j), own1 = min(((chunk + 1) * p.tk) << (K - j), half);
-            const int nbt = p.nb_top[j - 1], nbb = p.nb_bot[j - 1];
-            double* __restrict__ hib = p.hi[j - 1] + (int64_t)b * p.hi_stride[j - 1];
-            double* __restrict__ lob = p.lo + (int64_t)b * p.lo_stride;
-            const bool last = j == K;
-
-            // ---- interior outputs: tiles of 32 output positions x 2 bands, one warp per tile ----------------------
-            const int ntiles = (o1 - o0 + 31) / 32;
-            const int lo_all = max(nbt, o0), hi_all = min(half - nbb, o1);
-            // Tiles [t_lo, t_hi) are "fast": all 32 outputs are interior ones of this chunk and every sample of their
-            // windows is staged (the conditions are linear in the tile index, so the range is computed once per level).
-            int t_lo, t_hi;
-            {
-                const int need0 = max(lo_all - o0, (HL + SH + in0 + 1) / 2 - o0);          // first admissible i0 - o0
-                t_lo = need0 > 0 ? (need0 + 31) / 32 : 0;
-                const int lim_out = (hi_all - o0) / 32;                                     // i0 + 32 <= hi_all
-                const int lim_in = in_cnt - 56 - 4 * E + HL + SH + in0 - 2 * o0;            // 2 (i0 - o0) <= lim_in
-                t_hi = min(lim_out, lim_in >= 0 ? lim_in / 64 + 1 : 0);
-                t_hi = max(min(t_hi, ntiles), t_lo);
-            }
-            auto generic_tile = [&](const int t) {
-                const int i0 = o0 + 32 * t;
-                const int rel0 = 2 * i0 + 8 * frag_n - HL - SH + KS * frag_k - in0;
-                double c0 = 0.0, c1 = 0.0;
-                const int ia = i0 + 4 * out_g0 + out_s, ib = ia + 4;
-                // samples clamped into the staged range (only outputs that the corner-block code below overwrites, or
-                // that lie beyond o1, can touch the clamp), stores checked one by one
-#pragma unroll
-                for (int e = 0; e < E; ++e) {
-                    const int rel = min(max(rel0 + ES * e, 0), in_cnt - 1);
-                    dmma_m8n8k4(c0, c1, afrag[e], in[rel]);
-                }
-                if (out_band == 0) {
-                    if (!last) {
-                        if (ia < o1) nxt[ia - o0] = c0;
-                        if (ib < o1) nxt[ib - o0] = c1;
-                    } else {
-                        if (ia >= own0 && ia < own1 && ia >= nbt && ia < half - nbb) lob[ia] = c0;
-                        if (ib >= own0 && ib < own1 && ib >= nbt && ib < half - nbb) lob[ib] = c1;
-                    }
-                } else {
-                    if (ia >= own0 && ia < own1 && ia >= nbt && ia < half - nbb) hib[ia] = c0;
-                    if (ib >= own0 && ib < own1 && ib >= nbt && ib < half - nbb) hib[ib] = c1;
-                }
-            };
-            for (int t = warp; t < t_lo; t += NW) generic_tile(t);
-            for (int t = t_hi + warp; t < ntiles; t += NW) generic_tile(t);
-            {
-                // fast tiles: running pointers, no range checks besides the owned range of the global stores
-                const int tf = t_lo + warp;
-                int ia = o0 + 32 * tf + 4 * out_g0 + out_s;
-                const double* src = in + (2 * (o0 + 32 * tf) + 8 * frag_n - HL - SH + KS * frag_k - in0);
-                double* dsm = nxt + (ia - o0);
-                double* dgl = (out_band ? hib : lob) + ia;
-                const bool to_smem = out_band == 0 && !last;
-                for (int t = tf; t < t_hi; t += NW) {
-                    double c0 = 0.0, c1 = 0.0;
-                    if constexpr (PERM) {
-#pragma unroll
-                        for (int e = 0; e < E; e += 2) {
-                            const double2 v = *reinterpret_cast<const double2*>(src + e);
-                            dmma_m8n8k4(c0, c1, afrag[e], v.x);
-                            dmma_m8n8k4(c0, c1, afrag[e + 1], v.y);
-                        }
-                    } else {
-                        double v[E];
-#pragma unroll
-                        for (int e = 0; e < E; ++e) v[e] = src[4 * e];
-#pragma unroll
-                        for (int e = 0; e < E; ++e) dmma_m8n8k4(c0, c1, afrag[e], v[e]);
-                    }
-                    if (to_smem) {
-                        dsm[0] = c0; dsm[4] = c1;
-                    } else {
-                        if (ia >= own0 && ia < own1) dgl[0] = c0;
-                        if (ia + 4 >= own0 && ia + 4 < own1) dgl[4] = c1;
-                    }
-                    src += 64 * NW; dsm += 32 * NW; dgl += 32 * NW; ia += 32 * NW;
-                }
-            }
-            __syncthreads();
-            // ---- corner blocks: the dense orthogonalised boundary rows (the CTAs at the two ends of the row) -------
-            if (o0 < nbt || o1 > half - nbb) {
-                // outputs [o0, min(o1, nbt)) and [max(o0, half - nbb), o1), both bands
-                const int nt_ = max(min(o1, nbt) - o0, 0);
-                const int b0 = max(o0, half - nbb), nb_ = max(o1 - b0, 0);
-                for (int q = tid; q < 2 * (nt_ + nb_); q += NT) {
-                    const int band = q & 1, r = q >> 1;
-                    const int ii = r < nt_ ? o0 + r : b0 + (r - nt_);
-                    const bool top = ii < nbt;
-                    const int rr = top ? ii : nbt + (ii - (half - nbb));
-                    const int w = top ? p.w_left[j - 1] : p.w_right[j - 1];
-                    const int s0 = top ? 0 : nprev - w;
-                    const double* __restrict__ blk = (top ? (band ? p.hi_left[j - 1] : p.lo_left[j - 1])
-                                                          : (band ? p.hi_right[j - 1] : p.lo_right[j - 1])) + rr * w;
-                    double acc = 0.0;
-                    for (int c = 0; c < w; ++c) acc = fma(__ldg(blk + c), in[s0 + c - in0], acc);
-                    if (band == 0) {
-                        if (!last) nxt[ii - o0] = acc;
-                        else if (ii >= own0 && ii < own1) lob[ii] = acc;
-                    } else if (ii >= own0 && ii < own1) {
-                        hib[ii] = acc;
-                    }
-                }
-                __syncthreads();
-            }
-            in = nxt;
-            nxt = (nxt == levA) ? levB : levA;
-        }
-    }
-}
-
-// Host: launch one fused group of k levels on the FP64 tensor cores; false = not applicable (caller falls back).
-static bool launch_mat_fwd_dmma(int L, int k, const int64_t* n, const int32_t* nbt, const int32_t* nbb, const int32_t* wl,
-                                const int32_t* wr, const double* const* blk_ptrs, const double* x, int64_t xs, int64_t batch,
-                                void* const* hi_out, const int64_t* hi_stride, double* lo_out, int64_t lo_stride,
-                                const Taps<double>& taps, cudaStream_t st, cudaError_t* err) {
-    *err = cudaSuccess;
-    if ((L & 1) || L < 2 || L > 16 || k < 1 || k > MATF_MAXK || batch > 65535) return false;
-    if (((uintptr_t)x & 15) || (xs & 1) || n[0] >= (int64_t(1) << 30)) return false;
-    MatFusedParams<double> p;
-    memset(&p, 0, sizeof(p));
-    p.x = x; p.x_stride = xs; p.k = k;
-    p.n[0] = (int)n[0];
-    for (int j = 0; j < k; ++j) {
-        if (n[j] & 1) return false;
-        p.n[j + 1] = (int)(n[j] / 2);
-        if (j + 1 < k && n[j + 1] != n[j] / 2) return false;
-        p.hi[j] = (double*)hi_out[j]; p.hi_stride[j] = hi_stride[j];
-        p.nb_top[j] = nbt[j]; p.nb_bot[j] = nbb[j]; p.w_left[j] = wl[j]; p.w_right[j] = wr[j];
-        p.lo_left[j] = blk_ptrs[4 * j]; p.lo_right[j] = blk_ptrs[4 * j + 1];
-        p.hi_left[j] = blk_ptrs[4 * j + 2]; p.hi_right[j] = blk_ptrs[4 * j + 3];
-        if (nbt[j] + nbb[j] > p.n[j + 1]) return false;
-    }
-    p.lo = lo_out; p.lo_stride = lo_stride;
-    for (int q = 0; q < L; ++q) { p.flo[q] = taps.lo[L - 1 - q]; p.fhi[q] = taps.hi[L - 1 - q]; }
-    const int nk = p.n[k];
-    int chunk0 = 2048;
-    if (knob_is_set(K_MATF_CHUNK)) { const int v = (int)knob_val(K_MATF_CHUNK, 0); if (v >= 64 && v <= 16384) chunk0 = v; }
-    if (n[0] <= 8192 && n[0] > chunk0) chunk0 = (int)n[0];
-    int tk = chunk0 >> k;
-    if (tk < 4) tk = 4;
-    tk = (tk + 3) & ~3;
-    if (tk > nk) tk = (nk + 3) & ~3;
-    p.tk = tk;
-    int cap0 = (tk << k) + ((L + 6) << k) + 64;
-    if (cap0 > p.n[0] + 16) cap0 = (p.n[0] + 16 + 3) & ~3;
-    cap0 = (cap0 + 3) & ~3;
-    p.cap0 = cap0;
-    const size_t smem = (size_t)(2 * cap0 + (cap0 / 2 + 16) + (cap0 / 4 + 16)) * sizeof(double);
-    if (smem > 200 * 1024) return false;
-    const int nchunks = (nk + tk - 1) / tk;
-    int cpc = (int)knob_val(K_MATF_CPC, 8);
-    if (cpc < 1) cpc = 1;
-    const int64_t min_ctas = knob_val(K_MATF_MINCTAS, 4 * sm_count());
-    while (cpc > 1 && (int64_t)((nchunks + cpc - 1) / cpc) * batch < min_ctas) cpc /= 2;
-    p.cpc = cpc;
-    dim3 grid((nchunks + cpc - 1) / cpc, (unsigned)batch);
-    const int nt = knob_val(K_MATF_NT, 128) == 256 ? 256 : 128;
-    const bool perm = knob_on(K_DMMA_PERM);
-#define WTB_MD_LAUNCH(LL, NTT, PP)                                                                     \
-    {                                                                                                  \
-        cudaError_t e = ensure_dyn_smem(mat_fwd_dmma_kernel<LL, NTT, PP>, 200 * 1024);                 \
-        if (e != cudaSuccess) { *err = e; return true; }                                               \
-        mat_fwd_dmma_kernel<LL, NTT, PP><<<grid, NTT, smem, st>>>(p);                                  \
-    }
-#define WTB_MD(LL)                                                                                     \
-    case LL:                                                                                           \
-        if (nt == 128) { if (perm) WTB_MD_LAUNCH(LL, 128, true) else WTB_MD_LAUNCH(LL, 128, false) }      \
-        else { if (perm) WTB_MD_LAUNCH(LL, 256, true) else WTB_MD_LAUNCH(LL, 256, false) }                \
-        break;
-    switch (L) {
-        WTB_MD(2) WTB_MD(4) WTB_MD(6) WTB_MD(8) WTB_MD(10) WTB_MD(12) WTB_MD(14) WTB_MD(16)
-        default: return false;
-    }
-#undef WTB_MD
-#undef WTB_MD_LAUNCH
-    *err = cudaGetLastError();
-    return true;
-}
-
-
 // ==========================================================================================
-// The analysis cascade again, laid out like the synthesis kernel below (conflict-free polyphase operand loads, which
-// the kernel above lacks): one chunk per CTA, every level input kept as two POLYPHASE arrays
+// MatrixWavedec on the FP64 tensor cores: the analysis cascade of K levels in one launch, laid out like the synthesis
+// kernel below: one chunk per CTA, every level input kept as two POLYPHASE arrays
 // (even samples | odd samples, the odd array two doubles further in the bank pattern), the DATA in the A operand and
 // the polyphase FILTER matrix in the B operand:
 //
@@ -502,7 +227,8 @@ __global__ void __launch_bounds__(NT) mat_fwd_dmma2_kernel(const __grid_constant
     }
 }
 
-// Host: the polyphase analysis cascade; false = not applicable (caller falls back to the streaming kernel).
+// Host: the polyphase analysis cascade; false = not applicable (the caller runs mat_fwd_fused_kernel or the per-level
+// kernels instead).
 static bool launch_mat_fwd_dmma2(int L, int k, const int64_t* n, const int32_t* nbt, const int32_t* nbb, const int32_t* wl,
                                  const int32_t* wr, const double* const* blk_ptrs, const double* x, int64_t xs, int64_t batch,
                                  void* const* hi_out, const int64_t* hi_stride, double* lo_out, int64_t lo_stride,
@@ -511,25 +237,13 @@ static bool launch_mat_fwd_dmma2(int L, int k, const int64_t* n, const int32_t* 
     if ((L & 1) || L < 2 || L > 16 || k < 1 || k > MATF_MAXK || batch > 65535) return false;
     if (n[0] >= (int64_t(1) << 30)) return false;
     MatFusedParams<double> p;
-    memset(&p, 0, sizeof(p));
-    p.x = x; p.x_stride = xs; p.k = k;
-    p.n[0] = (int)n[0];
+    if (!fill_mat_fused_levels(p, L, k, n, nbt, nbb, wl, wr, blk_ptrs, x, xs, hi_out, hi_stride, lo_out, lo_stride, taps))
+        return false;
     int vec = 0;
     if (!((uintptr_t)lo_out & 15) && !(lo_stride & 1)) vec |= 1 << 15;
-    for (int j = 0; j < k; ++j) {
-        if (n[j] & 1) return false;
-        p.n[j + 1] = (int)(n[j] / 2);
-        if (j + 1 < k && n[j + 1] != n[j] / 2) return false;
-        p.hi[j] = (double*)hi_out[j]; p.hi_stride[j] = hi_stride[j];
+    for (int j = 0; j < k; ++j)
         if (!((uintptr_t)hi_out[j] & 15) && !(hi_stride[j] & 1)) vec |= 1 << j;
-        p.nb_top[j] = nbt[j]; p.nb_bot[j] = nbb[j]; p.w_left[j] = wl[j]; p.w_right[j] = wr[j];
-        p.lo_left[j] = blk_ptrs[4 * j]; p.lo_right[j] = blk_ptrs[4 * j + 1];
-        p.hi_left[j] = blk_ptrs[4 * j + 2]; p.hi_right[j] = blk_ptrs[4 * j + 3];
-        if (nbt[j] + nbb[j] > p.n[j + 1]) return false;
-    }
     p.vec = vec;
-    p.lo = lo_out; p.lo_stride = lo_stride;
-    for (int q = 0; q < L; ++q) { p.flo[q] = taps.lo[L - 1 - q]; p.fhi[q] = taps.hi[L - 1 - q]; }
     const int nk = p.n[k];
     int chunk0 = 2048;
     if (knob_is_set(K_MATF_CHUNK)) { const int v = (int)knob_val(K_MATF_CHUNK, 0); if (v >= 64 && v <= 16384) chunk0 = v; }
@@ -585,11 +299,34 @@ static bool launch_mat_fwd_dmma2(int L, int k, const int64_t* n, const int32_t* 
 // shared load per lane which is bank-conflict free because the detail band is staged two doubles behind the
 // approximation band.  W / 2 DMMAs + W / 2 loads + 1 store per 64 outputs (L = 12: 0.17 warp instructions per sample).
 //
-// The cascade around it is that of mat_inv_fused_kernel (matrix_fused.cuh): a CTA owns a chunk of the finest output,
-// stages every detail range and the coarsest approximation range by cp.async (one commit group per level, so the
-// coarse levels start while the fine details are still in flight), keeps every intermediate approximation in shared
-// memory, and the CTAs at the two ends apply the dense corner rows by scalar code.
+// The cascade around it: a CTA owns a chunk of the finest output, stages every detail range and the coarsest
+// approximation range by cp.async (one commit group per level, so the coarse levels start while the fine details are
+// still in flight), keeps every intermediate approximation in shared memory, and the CTAs at the two ends apply the
+// dense corner rows by scalar code.
 // ==========================================================================================
+template <typename T>
+struct MatInvFusedParams {
+    const T* lo;                 // approximation entering the coarsest fused level, [batch, n[K-1]/2]
+    int64_t lo_stride;
+    const T* hi[MATF_MAXK];      // hi[j-1]: detail of fused level j (j = 1 finest), [batch, n[j-1]/2]
+    int64_t hi_stride[MATF_MAXK];
+    T* y;                        // [batch, keep0]
+    int64_t y_stride;
+    int k;
+    int n[MATF_MAXK];            // n[j-1] = operator size of fused level j (its output length before trimming)
+    int keep0;                   // samples of the finest output that are stored (n[0] or n[0] - 1)
+    int nb_top[MATF_MAXK], nb_bot[MATF_MAXK], w_left[MATF_MAXK], w_right[MATF_MAXK];
+    const T* lo_left[MATF_MAXK];
+    const T* lo_right[MATF_MAXK];
+    const T* hi_left[MATF_MAXK];
+    const T* hi_right[MATF_MAXK];
+    int chunk;                   // finest-level samples per CTA (multiple of 64)
+    int cap;                     // capacity of one approximation buffer
+    int hi_cap;                  // capacity of the detail staging area
+    T rlo[16], rhi[16];          // rec_lo / rec_hi, un-flipped
+    int vec;                     // bit j-1 = hi[j-1] rows 16-byte aligned, bit 14 = y, bit 15 = lo
+};
+
 __device__ __forceinline__ void cp_async_wait_dyn(int pending) {
     switch (pending) {
         case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
@@ -796,242 +533,6 @@ __global__ void __launch_bounds__(NT) mat_inv_dmma_kernel(const __grid_constant_
     }
 }
 
-// ------------------------------------------------------------------------------------------
-// The same cascade, streaming ROWS: a CTA keeps its chunk index and walks p.rows batch rows.  The coefficient ranges
-// and tile ranges depend on the chunk only, so they are computed once; the next row's details and coarsest
-// approximation arrive by TMA bulk copies (cp.async.bulk, one mbarrier per level and buffer set) while the current row
-// is synthesised, which removes the per-thread staging loops and the per-level range arithmetic of the kernel above.
-// Needs 16-byte aligned rows and even band lengths (bulk copies move multiples of 16 bytes).
-// ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void md_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(count));
-}
-__device__ __forceinline__ void md_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)),
-                 "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void md_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "MD_WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra MD_DONE;\n\t"
-        "bra MD_WAIT_LOOP;\n\t"
-        "MD_DONE:\n\t"
-        "}" ::"r"((uint32_t)__cvta_generic_to_shared(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void md_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     (uint32_t)__cvta_generic_to_shared(dst)),
-                 "l"(src), "r"(bytes), "r"((uint32_t)__cvta_generic_to_shared(bar))
-                 : "memory");
-}
-
-enum { MDI_A = 0, MDI_BND, MDI_C0, MDI_CNT, MDI_STOP, MDI_SBOT, MDI_TL0, MDI_TL1, MDI_FLO, MDI_FHI, MDI_N };
-
-template <int L, int NT>
-__global__ void __launch_bounds__(NT) mat_inv_dmma_rows_kernel(const __grid_constant__ MatInvFusedParams<double> p) {
-    constexpr int H = L / 2;
-    constexpr int C = H / 2;
-    constexpr int KS = C + 2;
-    constexpr int W = 2 * KS;
-    constexpr int NW = NT / 32;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    double* bufA = reinterpret_cast<double*>(smem_raw);
-    double* bufB = bufA + p.cap;
-    double* lost = bufB + p.cap;                  // [2][cap_lo]  coarsest approximation of the current / next row
-    double* hist = lost + 2 * p.cap_lo + 2;       // [2][hi_cap]  details, two doubles behind (bank note above)
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int K = p.k;
-    if ((int64_t)blockIdx.x * p.chunk >= p.keep0) return;
-    const int row0 = blockIdx.y * p.rows;
-    const int nrows = min(p.rows, p.batch - row0);
-
-    __shared__ int s_info[MATF_MAXK][MDI_N];
-    __shared__ int s_hoff[MATF_MAXK + 1];
-    __shared__ __align__(8) uint64_t s_bar[2][MATF_MAXK];
-    if (tid == 0) {
-        int ra = blockIdx.x * p.chunk, rb = min(ra + p.chunk, p.n[0]), ho = 0;
-        s_hoff[0] = 0;
-        for (int j = 1; j <= K; ++j) {
-            const int nout = p.n[j - 1], N = nout / 2;
-            const int nbt = p.nb_top[j - 1], nbb = p.nb_bot[j - 1], wl = p.w_left[j - 1], wr = p.w_right[j - 1];
-            const int a = ra, bnd = rb;
-            int ia = (a - H + 1) >> 1;
-            int ib = (bnd - 1 + H - 1) >> 1;
-            if (a < wl) { ia = 0; ib = max(ib, nbt - 1); }
-            if (bnd > nout - wr) { ib = N - 1; ia = min(ia, N - nbb); }
-            ra = max(ia, 0) & ~3;
-            rb = min((ib + 2) & ~1, N);                                 // even count: bulk copies move 16-byte units
-            const int c0 = ra, cnt = rb - ra;
-            ho += (cnt + 3) & ~3;
-            s_hoff[j] = ho;
-            const int s_top = min(max(max(wl, 2 * nbt + H), a), bnd);
-            const int s_bot = max(min(min(nout - wr, 2 * (N - nbb) - H), bnd), s_top);
-            const int tl_first = (s_top - a) >> 6, tl_end = (s_bot - a + 63) >> 6;
-            const int need = max(s_top - a, 2 * (c0 + C) - a);
-            int f_lo = need > 0 ? (need + 63) >> 6 : 0;
-            const int lim_in = 2 * (cnt + c0 + C - W - 28) - a;
-            int f_hi = min((s_bot - a) >> 6, lim_in >= 0 ? (lim_in >> 6) + 1 : 0);
-            f_lo = min(max(f_lo, tl_first), tl_end);
-            f_hi = min(max(f_hi, f_lo), tl_end);
-            int* o = s_info[j - 1];
-            o[MDI_A] = a; o[MDI_BND] = bnd; o[MDI_C0] = c0; o[MDI_CNT] = cnt; o[MDI_STOP] = s_top; o[MDI_SBOT] = s_bot;
-            o[MDI_TL0] = tl_first; o[MDI_TL1] = tl_end; o[MDI_FLO] = f_lo; o[MDI_FHI] = f_hi;
-        }
-        for (int q = 0; q < 2 * MATF_MAXK; ++q) md_mbar_init(&s_bar[0][0] + q, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    auto issue = [&](const int row, const int set) {                  // one thread
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of this set precede the refill
-        for (int j = K; j >= 1; --j) {
-            const int c0 = s_info[j - 1][MDI_C0], cnt = s_info[j - 1][MDI_CNT];
-            uint64_t* bar = &s_bar[set][j - 1];
-            md_mbar_expect_tx(bar, (uint32_t)cnt * 8u * (j == K ? 2u : 1u));
-            if (j == K) md_bulk_g2s(lost + set * p.cap_lo, p.lo + (int64_t)row * p.lo_stride + c0, (uint32_t)cnt * 8u, bar);
-            md_bulk_g2s(hist + set * p.hi_cap + s_hoff[j - 1], p.hi[j - 1] + (int64_t)row * p.hi_stride[j - 1] + c0,
-                        (uint32_t)cnt * 8u, bar);
-        }
-    };
-    if (tid == 0) issue(row0, 0);
-
-    double bfrag[KS];
-    {
-        const int s = lane >> 2, k = lane & 3;
-#pragma unroll
-        for (int e = 0; e < KS; ++e) {
-            const int w = 2 * e + (k >> 1);
-            const int kk = s + H - 1 + 2 * C - 2 * w;
-            bfrag[e] = (kk >= 0 && kk < L) ? ((k & 1) ? p.rhi[kk] : p.rlo[kk]) : 0.0;
-        }
-    }
-    const int a_off = 4 * (lane >> 2) + ((lane & 3) >> 1) - C;
-    const bool a_hi = lane & 1;
-    const bool vec_y = (p.vec >> 14) & 1;
-
-#pragma unroll 1
-    for (int r = 0; r < nrows; ++r) {
-        const int set = r & 1;
-        const uint32_t par = (r >> 1) & 1;
-        if (tid == 0 && r + 1 < nrows) issue(row0 + r + 1, set ^ 1);
-        double* __restrict__ yb = p.y + (int64_t)(row0 + r) * p.y_stride;
-        const double* cur = lost + set * p.cap_lo;
-        double* nxt = bufA;
-#pragma unroll 1
-        for (int j = K; j >= 1; --j) {
-            const int* o = s_info[j - 1];
-            const int a = o[MDI_A], bnd = o[MDI_BND], c0 = o[MDI_C0], cnt = o[MDI_CNT];
-            const int s_top = o[MDI_STOP], s_bot = o[MDI_SBOT];
-            const int tl_first = o[MDI_TL0], tl_end = o[MDI_TL1], f_lo = o[MDI_FLO], f_hi = o[MDI_FHI];
-            const double* sl = cur;
-            const double* sh = hist + set * p.hi_cap + s_hoff[j - 1];
-            const bool last = j == 1;
-            const int lim = last ? min(bnd, p.keep0) : bnd;
-
-            md_mbar_wait(&s_bar[set][j - 1], par);
-            __syncthreads();                       // the coarser level's samples are complete
-
-            const double* band = a_hi ? sh : sl;
-            auto generic_tile = [&](const int t) {
-                const int t0 = a + 64 * t;
-                const int rel0 = (t0 >> 1) + a_off - c0;
-                double d0 = 0.0, d1 = 0.0;
-#pragma unroll
-                for (int e = 0; e < KS; ++e) {
-                    const int rel = min(max(rel0 + 2 * e, 0), cnt - 1);
-                    dmma_m8n8k4(d0, d1, band[rel], bfrag[e]);
-                }
-                const int ta = t0 + 2 * lane;
-                if (!last) {
-                    if (ta >= s_top && ta < s_bot) nxt[ta - a] = d0;
-                    if (ta + 1 >= s_top && ta + 1 < s_bot) nxt[ta + 1 - a] = d1;
-                } else {
-                    if (ta >= s_top && ta < s_bot && ta < lim) yb[ta] = d0;
-                    if (ta + 1 >= s_top && ta + 1 < s_bot && ta + 1 < lim) yb[ta + 1] = d1;
-                }
-            };
-            for (int t = tl_first + warp; t < f_lo; t += NW) generic_tile(t);
-            for (int t = f_hi + warp; t < tl_end; t += NW) generic_tile(t);
-            {
-                const int tf = f_lo + warp;
-                const double* src = band + (((a + 64 * tf) >> 1) + a_off - c0);
-                if (!last) {
-                    double* dsm = nxt + 64 * tf + 2 * lane;
-                    for (int t = tf; t < f_hi; t += NW) {
-                        double v[KS];
-#pragma unroll
-                        for (int e = 0; e < KS; ++e) v[e] = src[2 * e];
-                        double d0 = 0.0, d1 = 0.0;
-#pragma unroll
-                        for (int e = 0; e < KS; ++e) dmma_m8n8k4(d0, d1, v[e], bfrag[e]);
-                        *reinterpret_cast<double2*>(dsm) = make_double2(d0, d1);
-                        src += 32 * NW; dsm += 64 * NW;
-                    }
-                } else {
-                    double* dgl = yb + a + 64 * tf + 2 * lane;
-                    for (int t = tf; t < f_hi; t += NW) {
-                        double v[KS];
-#pragma unroll
-                        for (int e = 0; e < KS; ++e) v[e] = src[2 * e];
-                        double d0 = 0.0, d1 = 0.0;
-#pragma unroll
-                        for (int e = 0; e < KS; ++e) dmma_m8n8k4(d0, d1, v[e], bfrag[e]);
-                        if (vec_y) {
-                            *reinterpret_cast<double2*>(dgl) = make_double2(d0, d1);
-                        } else {
-                            dgl[0] = d0; dgl[1] = d1;
-                        }
-                        src += 32 * NW; dgl += 64 * NW;
-                    }
-                }
-            }
-            const int ntop = s_top - a, nbot = bnd - s_bot;
-            if (ntop + nbot > 0) {
-                const int nout = p.n[j - 1], N = nout / 2;
-                const int nbt = p.nb_top[j - 1], nbb = p.nb_bot[j - 1], wl = p.w_left[j - 1], wr = p.w_right[j - 1];
-                for (int q = tid; q < ntop + nbot; q += NT) {
-                    const int t = q < ntop ? a + q : s_bot + (q - ntop);
-                    double acc = 0.0;
-                    int i0 = (t - H + 1) >> 1, i1 = (t + H - 1) >> 1;
-                    i0 = max(i0, nbt);
-                    i1 = min(i1, N - nbb - 1);
-                    for (int i = i0; i <= i1; ++i) {
-                        const int kk = t + H - 1 - 2 * i;
-                        acc = fma(p.rlo[kk], sl[i - c0], acc);
-                        acc = fma(p.rhi[kk], sh[i - c0], acc);
-                    }
-                    if (t < wl) {
-                        for (int rr = 0; rr < nbt; ++rr) {
-                            acc = fma(__ldg(p.lo_left[j - 1] + rr * wl + t), sl[rr - c0], acc);
-                            acc = fma(__ldg(p.hi_left[j - 1] + rr * wl + t), sh[rr - c0], acc);
-                        }
-                    }
-                    if (t >= nout - wr) {
-                        const int c = t - (nout - wr);
-                        for (int rr = nbt; rr < nbt + nbb; ++rr) {
-                            const int i = N - nbb + (rr - nbt);
-                            acc = fma(__ldg(p.lo_right[j - 1] + rr * wr + c), sl[i - c0], acc);
-                            acc = fma(__ldg(p.hi_right[j - 1] + rr * wr + c), sh[i - c0], acc);
-                        }
-                    }
-                    if (!last) nxt[t - a] = acc;
-                    else if (t < lim) yb[t] = acc;
-                }
-            }
-            cur = nxt;
-            nxt = (nxt == bufA) ? bufB : bufA;
-        }
-        __syncthreads();                           // this row's buffers are free: the next refill may start
-    }
-}
-
 // Host: one fused synthesis group on the FP64 tensor cores.  Arrays are indexed by fused level j-1 (0 = finest).
 static bool launch_mat_inv_dmma(int L, int k, const int64_t* n, int64_t keep0, const int32_t* nbt, const int32_t* nbb,
                                 const int32_t* wl, const int32_t* wr, const double* const* blk_ptrs /* 4 per level */,
@@ -1083,46 +584,9 @@ static bool launch_mat_inv_dmma(int L, int k, const int64_t* n, int64_t keep0, c
     }
     p.cap = cap; p.hi_cap = hcap;
     const int nt = knob_val(K_MATI_NT, 128) == 256 ? 256 : 128;
-    const unsigned nchunks = (unsigned)((keep0 + chunk - 1) / chunk);
-    // row-streaming kernel (TMA bulk staging): every source row 16-byte aligned, every band length even
-    bool rows_ok = (vec & (1 << 15)) != 0;
-    for (int j = 0; j < k; ++j) rows_ok = rows_ok && ((vec >> j) & 1) && !(n[j] & 3);
-    // WTB200_MATI_ROWS: > 0 = upper bound (lowered until two full waves of CTAs remain), < 0 = exactly that many,
-    // 0 = the chunk-per-CTA kernel
-    int rows = (int)knob_val(K_MATI_ROWS, 0);
-    const bool forced = rows < 0;
-    if (forced) rows = -rows;
-    if (rows > 64) rows = 64;
-    if (!forced)
-        while (rows > 1 && (int64_t)nchunks * ((batch + rows - 1) / rows) < 8 * sm_count()) rows /= 2;
-    p.rows = rows; p.batch = (int)batch; p.cap_lo = len;           // len = capacity of the coarsest range
-    const size_t smem_rows = (size_t)(2 * cap + 2 * len + 2 * hcap + 4) * sizeof(double);
-    if (rows_ok && rows >= 1 && smem_rows <= 200 * 1024 && batch < (int64_t(1) << 31)) {
-        dim3 grid(nchunks, (unsigned)((batch + rows - 1) / rows));
-        if (grid.y <= 65535) {
-#define WTB_MIR_LAUNCH(LL, NTT)                                                                        \
-    {                                                                                                  \
-        cudaError_t e = ensure_dyn_smem(mat_inv_dmma_rows_kernel<LL, NTT>, 200 * 1024);                \
-        if (e != cudaSuccess) { *err = e; return true; }                                               \
-        mat_inv_dmma_rows_kernel<LL, NTT><<<grid, NTT, smem_rows, st>>>(p);                            \
-    }
-#define WTB_MIR(LL)                                                                                    \
-    case LL:                                                                                           \
-        if (nt == 128) WTB_MIR_LAUNCH(LL, 128) else WTB_MIR_LAUNCH(LL, 256)                            \
-        break;
-            switch (L) {
-                WTB_MIR(2) WTB_MIR(4) WTB_MIR(6) WTB_MIR(8) WTB_MIR(10) WTB_MIR(12) WTB_MIR(14) WTB_MIR(16)
-                default: return false;
-            }
-#undef WTB_MIR
-#undef WTB_MIR_LAUNCH
-            *err = cudaGetLastError();
-            return true;
-        }
-    }
     const size_t smem = (size_t)(2 * cap + hcap + 4) * sizeof(double);
     if (smem > 200 * 1024) return false;
-    dim3 grid(nchunks, (unsigned)batch);
+    dim3 grid((unsigned)((keep0 + chunk - 1) / chunk), (unsigned)batch);
 #define WTB_MID_LAUNCH(LL, NTT)                                                                        \
     {                                                                                                  \
         cudaError_t e = ensure_dyn_smem(mat_inv_dmma_kernel<LL, NTT>, 200 * 1024);                     \

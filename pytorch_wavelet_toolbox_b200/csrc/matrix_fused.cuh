@@ -1,4 +1,5 @@
-// matrix_fused.cuh -- several levels of the boundary-filter matrix FWT in ONE kernel.
+// matrix_fused.cuh -- several analysis levels of the boundary-filter matrix FWT in ONE kernel (float32, and float64
+// with NO_DMMA; the float64 default is matrix_dmma.cuh).
 //
 // The reference applies one sparse operator per level (torch.sparse.mm, src/ptwt/matmul_transform.py:
 // 409-425), so every approximation vector makes a round trip through memory: 2x the compulsory traffic
@@ -256,16 +257,14 @@ __global__ void __launch_bounds__(NT, MINB) mat_fwd_fused_kernel(const __grid_co
 }
 
 
-// Host: launch one fused group of k levels (level indices l .. l+k-1 of the caller's arrays).
+// Host: fill the levels of one analysis group (level indices l .. l+k-1 of the caller's arrays) for either cascade
+// launcher, launch_mat_fwd_fused below or launch_mat_fwd_dmma2 (matrix_dmma.cuh).  false = the group is not one
+// cascade (odd or trimmed lengths inside it, or corner blocks that meet).
 template <typename T>
-static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* nbt, const int32_t* nbb, const int32_t* wl,
-                                 const int32_t* wr, const T* const* blk_ptrs /* 4 per level */, const T* x, int64_t xs,
-                                 int64_t batch, void* const* hi_out, const int64_t* hi_stride, T* lo_out, int64_t lo_stride,
-                                 const Taps<T>& taps, cudaStream_t st, cudaError_t* err) {
-    *err = cudaSuccess;
-    if ((L & 1) || L < 2 || L > 16 || k < 2 || k > MATF_MAXK || batch > 65535) return false;
-    if (((uintptr_t)x & 15) || (xs & 1) || n[0] >= (int64_t(1) << 30)) return false;
-    MatFusedParams<T> p;
+static bool fill_mat_fused_levels(MatFusedParams<T>& p, int L, int k, const int64_t* n, const int32_t* nbt,
+                                  const int32_t* nbb, const int32_t* wl, const int32_t* wr,
+                                  const T* const* blk_ptrs /* 4 per level */, const T* x, int64_t xs, void* const* hi_out,
+                                  const int64_t* hi_stride, T* lo_out, int64_t lo_stride, const Taps<T>& taps) {
     memset(&p, 0, sizeof(p));
     p.x = x; p.x_stride = xs; p.k = k;
     p.n[0] = (int)n[0];
@@ -281,6 +280,21 @@ static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* 
     }
     p.lo = lo_out; p.lo_stride = lo_stride;
     for (int q = 0; q < L; ++q) { p.flo[q] = taps.lo[L - 1 - q]; p.fhi[q] = taps.hi[L - 1 - q]; }
+    return true;
+}
+
+// Host: launch one fused group of k levels.
+template <typename T>
+static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* nbt, const int32_t* nbb, const int32_t* wl,
+                                 const int32_t* wr, const T* const* blk_ptrs /* 4 per level */, const T* x, int64_t xs,
+                                 int64_t batch, void* const* hi_out, const int64_t* hi_stride, T* lo_out, int64_t lo_stride,
+                                 const Taps<T>& taps, cudaStream_t st, cudaError_t* err) {
+    *err = cudaSuccess;
+    if ((L & 1) || L < 2 || L > 16 || k < 2 || k > MATF_MAXK || batch > 65535) return false;
+    if (((uintptr_t)x & 15) || (xs & 1) || n[0] >= (int64_t(1) << 30)) return false;
+    MatFusedParams<T> p;
+    if (!fill_mat_fused_levels(p, L, k, n, nbt, nbb, wl, wr, blk_ptrs, x, xs, hi_out, hi_stride, lo_out, lo_stride, taps))
+        return false;
     const int nk = p.n[k];
     int chunk0 = sizeof(T) == 8 ? 2048 : 4096;                    // level-0 samples per chunk
     if (knob_is_set(K_MATF_CHUNK)) { const int v = (int)knob_val(K_MATF_CHUNK, 0); if (v >= 64 && v <= 16384) chunk0 = v; }
@@ -325,232 +339,6 @@ static bool launch_mat_fwd_fused(int L, int k, const int64_t* n, const int32_t* 
     }
 #undef WTB_MF_LAUNCH
 #undef WTB_MF
-    *err = cudaGetLastError();
-    return true;
-}
-
-// ==========================================================================================
-// Synthesis: several levels of  y = S [lo; hi]  (reference src/ptwt/matmul_transform.py:682-699) in ONE kernel.
-//
-// A CTA owns a chunk of the group's finest output and, going up, the coefficient ranges of the coarser
-// levels it depends on (about L/4 coefficients of halo per side and level).  All detail ranges and the
-// coarsest approximation range are staged in shared memory first; then the levels are synthesised from
-// coarse to fine, every intermediate approximation staying in shared memory; only the finest level
-// writes to HBM.  A thread produces 4 consecutive samples from one window of both bands.
-// Boundary: the dense corner blocks are applied by the CTAs at the two ends; the round-off sized
-// cross-corner entries are dropped exactly as in the fused analysis kernel (same host-side criterion).
-// ==========================================================================================
-template <typename T>
-struct MatInvFusedParams {
-    const T* lo;                 // approximation entering the coarsest fused level, [batch, n[K-1]/2]
-    int64_t lo_stride;
-    const T* hi[MATF_MAXK];      // hi[j-1]: detail of fused level j (j = 1 finest), [batch, n[j-1]/2]
-    int64_t hi_stride[MATF_MAXK];
-    T* y;                        // [batch, keep0]
-    int64_t y_stride;
-    int k;
-    int n[MATF_MAXK];            // n[j-1] = operator size of fused level j (its output length before trimming)
-    int keep0;                   // samples of the finest output that are stored (n[0] or n[0] - 1)
-    int nb_top[MATF_MAXK], nb_bot[MATF_MAXK], w_left[MATF_MAXK], w_right[MATF_MAXK];
-    const T* lo_left[MATF_MAXK];
-    const T* lo_right[MATF_MAXK];
-    const T* hi_left[MATF_MAXK];
-    const T* hi_right[MATF_MAXK];
-    int chunk;                   // finest-level samples per CTA (multiple of 4 << k)
-    int cap;                     // capacity of one approximation buffer
-    int hi_cap;                  // capacity of the detail staging area
-    T rlo[16], rhi[16];          // rec_lo / rec_hi, un-flipped
-    int vec;                     // matrix_dmma.cuh: bit j-1 = hi[j-1] rows 16-byte aligned, bit 14 = y, bit 15 = lo
-    int rows, batch, cap_lo;     // matrix_dmma.cuh (row-streaming kernel): rows per CTA, batch, coarsest staging size
-};
-
-template <typename T, int L>
-__global__ void __launch_bounds__(256) mat_inv_fused_kernel(const __grid_constant__ MatInvFusedParams<T> p) {
-    constexpr int H = L / 2;
-    constexpr int C = (L / 4);                                     // window starts at t0/2 - C
-    constexpr int NCW = C + (4 + H - 2) / 2 + 1;                   // coefficients in the window of 4 samples
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    T* bufA = reinterpret_cast<T*>(smem_raw);
-    T* bufB = bufA + p.cap;
-    T* shi = bufB + p.cap;
-
-    const int tid = threadIdx.x;
-    const int b = blockIdx.y;
-    const int K = p.k;
-
-    // ranges: level-j coefficients [ra[j], rb[j]) needed (j >= 1); [ra[0], rb[0]) = samples this CTA writes
-    int ra[MATF_MAXK + 1], rb[MATF_MAXK + 1], hoff[MATF_MAXK + 1];
-    ra[0] = blockIdx.x * p.chunk;
-    rb[0] = min(ra[0] + p.chunk, p.n[0]);
-    if (ra[0] >= p.keep0) return;
-    hoff[0] = 0;
-#pragma unroll
-    for (int j = 1; j <= MATF_MAXK; ++j) {
-        if (j > K) continue;
-        const int nout = p.n[j - 1], N = nout / 2;
-        int ia = (ra[j - 1] - H + 1) >> 1;                         // ceil((a - L/2) / 2)
-        int ib = (rb[j - 1] - 1 + H - 1) >> 1;                     // floor((b - 1 + L/2 - 1) / 2)
-        if (ra[j - 1] < p.w_left[j - 1]) { ia = 0; ib = max(ib, p.nb_top[j - 1] - 1); }
-        if (rb[j - 1] > nout - p.w_right[j - 1]) { ib = N - 1; ia = min(ia, N - p.nb_bot[j - 1]); }
-        ra[j] = max(ia, 0) & ~3;
-        rb[j] = min(ib + 1, N);
-        hoff[j] = hoff[j - 1] + ((rb[j] - ra[j] + 3) & ~3);
-    }
-
-    // stage every detail range and the coarsest approximation range
-#pragma unroll
-    for (int j = 1; j <= MATF_MAXK; ++j) {
-        if (j > K) continue;
-        const T* __restrict__ hb = p.hi[j - 1] + (int64_t)b * p.hi_stride[j - 1] + ra[j];
-        T* dst = shi + hoff[j - 1];
-        const int cnt = rb[j] - ra[j];
-        for (int q = tid; q < cnt; q += 256) dst[q] = __ldg(hb + q);
-    }
-    {
-        const T* __restrict__ lb = p.lo + (int64_t)b * p.lo_stride + ra[K];
-        const int cnt = rb[K] - ra[K];
-        for (int q = tid; q < cnt; q += 256) bufA[q] = __ldg(lb + q);
-    }
-    __syncthreads();
-
-    T* cur = bufA;
-    T* nxt = bufB;
-#pragma unroll 1
-    for (int j = K; j >= 1; --j) {
-        const int nout = p.n[j - 1], N = nout / 2;
-        const int a = ra[j - 1], bnd = rb[j - 1];
-        const int c0 = ra[j], c1 = rb[j];                          // coefficient range held in shared memory
-        const T* sl = cur;
-        const T* sh = shi + hoff[j - 1];
-        const int nbt = p.nb_top[j - 1], nbb = p.nb_bot[j - 1], wl = p.w_left[j - 1], wr = p.w_right[j - 1];
-        T* __restrict__ yb = p.y + (int64_t)b * p.y_stride;
-        const int ngrp = (bnd - a + 3) >> 2;
-        for (int g = tid; g < ngrp; g += 256) {
-            const int t0 = a + 4 * g;
-            const int ilo = t0 / 2 - C;
-            T out[4];
-            const bool fast = ilo >= nbt && ilo >= c0 && ilo + NCW <= N - nbb && ilo + NCW <= c1 && t0 >= wl &&
-                              t0 + 4 <= nout - wr;
-            if (fast) {
-                T av[NCW], dv[NCW];
-#pragma unroll
-                for (int w = 0; w < NCW; ++w) { av[w] = sl[ilo - c0 + w]; dv[w] = sh[ilo - c0 + w]; }
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    T acc = T(0);
-#pragma unroll
-                    for (int w = 0; w < NCW; ++w) {
-                        const int kk = e + H - 1 + 2 * C - 2 * w;  // rec index for sample t0 + e, coefficient ilo + w
-                        if (kk >= 0 && kk < L) {
-                            acc = fma(p.rlo[kk], av[w], acc);
-                            acc = fma(p.rhi[kk], dv[w], acc);
-                        }
-                    }
-                    out[e] = acc;
-                }
-            } else {
-                for (int e = 0; e < 4; ++e) {
-                    const int t = t0 + e;
-                    T acc = T(0);
-                    if (t < nout) {
-                        int i0 = (t - H + 1) >> 1, i1 = (t + H - 1) >> 1;
-                        i0 = max(i0, nbt);
-                        i1 = min(i1, N - nbb - 1);
-                        for (int i = i0; i <= i1; ++i) {
-                            const int kk = t + H - 1 - 2 * i;
-                            acc = fma(p.rlo[kk], sl[i - c0], acc);
-                            acc = fma(p.rhi[kk], sh[i - c0], acc);
-                        }
-                        if (t < wl) {
-                            // top boundary rows only: the bottom rows' entries in the left corner are the dropped
-                            // cross-corner round-off (rows r >= nbt of the left block)
-                            for (int r = 0; r < nbt; ++r) {
-                                acc = fma(__ldg(p.lo_left[j - 1] + r * wl + t), sl[r - c0], acc);
-                                acc = fma(__ldg(p.hi_left[j - 1] + r * wl + t), sh[r - c0], acc);
-                            }
-                        }
-                        if (t >= nout - wr) {
-                            const int c = t - (nout - wr);
-                            for (int r = nbt; r < nbt + nbb; ++r) {
-                                const int i = N - nbb + (r - nbt);
-                                acc = fma(__ldg(p.lo_right[j - 1] + r * wr + c), sl[i - c0], acc);
-                                acc = fma(__ldg(p.hi_right[j - 1] + r * wr + c), sh[i - c0], acc);
-                            }
-                        }
-                    }
-                    out[e] = acc;
-                }
-            }
-            if (j > 1) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) nxt[t0 - a + e] = out[e];
-            } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                    if (t0 + e < p.keep0 && t0 + e < bnd) yb[t0 + e] = out[e];
-            }
-        }
-        __syncthreads();
-        T* tswap = cur; cur = nxt; nxt = tswap;
-    }
-}
-
-// Host: one fused synthesis group.  Arrays are indexed by fused level j-1 (0 = finest of the group).
-template <typename T>
-static bool launch_mat_inv_fused(int L, int k, const int64_t* n, int64_t keep0, const int32_t* nbt, const int32_t* nbb,
-                                 const int32_t* wl, const int32_t* wr, const T* const* blk_ptrs /* 4 per level */,
-                                 const T* lo, int64_t lo_stride, const void* const* hi_in, const int64_t* hi_stride,
-                                 int64_t batch, T* y, int64_t y_stride, const double* rlo, const double* rhi, cudaStream_t st,
-                                 cudaError_t* err) {
-    *err = cudaSuccess;
-    if ((L & 1) || L < 2 || L > 16 || k < 2 || k > MATF_MAXK || batch > 65535) return false;
-    if (n[0] >= (int64_t(1) << 30)) return false;
-    MatInvFusedParams<T> p;
-    memset(&p, 0, sizeof(p));
-    p.lo = lo; p.lo_stride = lo_stride; p.y = y; p.y_stride = y_stride; p.k = k;
-    p.keep0 = (int)keep0;
-    for (int j = 0; j < k; ++j) {
-        if (n[j] & 1) return false;
-        if (j + 1 < k && n[j + 1] != n[j] / 2) return false;       // no trimming inside a group
-        p.n[j] = (int)n[j];
-        p.hi[j] = (const T*)hi_in[j]; p.hi_stride[j] = hi_stride[j];
-        p.nb_top[j] = nbt[j]; p.nb_bot[j] = nbb[j]; p.w_left[j] = wl[j]; p.w_right[j] = wr[j];
-        p.lo_left[j] = blk_ptrs[4 * j]; p.lo_right[j] = blk_ptrs[4 * j + 1];
-        p.hi_left[j] = blk_ptrs[4 * j + 2]; p.hi_right[j] = blk_ptrs[4 * j + 3];
-        if (nbt[j] + nbb[j] > n[j] / 2) return false;
-    }
-    for (int q = 0; q < L; ++q) { p.rlo[q] = (T)rlo[q]; p.rhi[q] = (T)rhi[q]; }
-    int chunk = sizeof(T) == 8 ? 2048 : 4096;
-    if (knob_is_set(K_MATI_CHUNK)) { const int v = (int)knob_val(K_MATI_CHUNK, 0); if (v >= 64 && v <= 16384) chunk = v; }
-    const int gran = 4 << k;
-    chunk = (chunk + gran - 1) / gran * gran;
-    if (chunk > p.n[0]) chunk = (p.n[0] + gran - 1) / gran * gran;
-    p.chunk = chunk;
-    // per level the range grows by at most L/2 + 4 coefficients (halo + alignment) + the corner rows
-    int cap = 0, hcap = 0, len = chunk;
-    for (int j = 0; j < k; ++j) {
-        len = len / 2 + L / 2 + 8 + nbt[j] + nbb[j] + std::max(wl[j], wr[j]);
-        if (len > p.n[j] / 2 + 4) len = p.n[j] / 2 + 4;
-        len = (len + 3) & ~3;
-        cap = std::max(cap, len);
-        hcap += len;
-    }
-    p.cap = cap; p.hi_cap = hcap;
-    const size_t smem = (size_t)(2 * cap + hcap) * sizeof(T);
-    if (smem > 200 * 1024) return false;
-    dim3 grid((unsigned)((keep0 + chunk - 1) / chunk), (unsigned)batch);
-#define WTB_MIF(LL)                                                                                             \
-    case LL: {                                                                                                  \
-        cudaError_t e = ensure_dyn_smem(mat_inv_fused_kernel<T, LL>, smem > 200 * 1024 ? smem : 200 * 1024);         \
-        if (e != cudaSuccess) { *err = e; return true; }                                                        \
-        mat_inv_fused_kernel<T, LL><<<grid, 256, smem, st>>>(p);                                                \
-        break;                                                                                                  \
-    }
-    switch (L) {
-        WTB_MIF(2) WTB_MIF(4) WTB_MIF(6) WTB_MIF(8) WTB_MIF(10) WTB_MIF(12) WTB_MIF(14) WTB_MIF(16)
-        default: return false;
-    }
-#undef WTB_MIF
     *err = cudaGetLastError();
     return true;
 }

@@ -554,16 +554,12 @@ static int matrix_fwd_t(int levels, int L, const double* dlo, const double* dhi,
                 cudaError_t e = cudaSuccess;
                 bool launched = false;
                 if constexpr (sizeof(T) == 8) {
-                    // float64: the band contraction on the FP64 tensor cores (matrix_dmma.cuh)
-                    // (matrix_dmma.cuh: the polyphase kernel, WTB200_MATF_VARIANT=1 = the streaming kernel)
-                    if (!knob_on(K_NO_DMMA) && knob_val(K_MATF_VARIANT, 2) != 1)
+                    // float64: the polyphase band contraction on the FP64 tensor cores (matrix_dmma.cuh); the scalar
+                    // cascade below where it does not apply
+                    if (dmma64)
                         launched = launch_mat_fwd_dmma2(L, k, n + l, nbt + l, nbb + l, wt + l, wb + l,
                                                         (const double* const*)(bptr + 4 * l), (const double*)src, src_stride, batch,
                                                         hi_out + l, hi_stride + l, (double*)lo_dst, lo_ds, taps, st, &e);
-                    if (!launched && !knob_on(K_NO_DMMA))
-                        launched = launch_mat_fwd_dmma(L, k, n + l, nbt + l, nbb + l, wt + l, wb + l,
-                                                       (const double* const*)(bptr + 4 * l), (const double*)src, src_stride, batch,
-                                                       hi_out + l, hi_stride + l, (double*)lo_dst, lo_ds, taps, st, &e);
                 }
                 if (launched ||
                     launch_mat_fwd_fused<T>(L, k, n + l, nbt + l, nbb + l, wt + l, wb + l, bptr + 4 * l, src, src_stride, batch,
@@ -652,19 +648,19 @@ static int matrix_inv_t(int levels, int L, const double* rlo, const double* rhi,
         bptr[4 * l + 2] = q; q += nb * wt[l];
         bptr[4 * l + 3] = q;
     }
+    // float64: groups of levels run as one synthesis cascade on the FP64 tensor cores (matrix_dmma.cuh).  float32 (and
+    // float64 with NO_DMMA) runs the register-blocked per-level kernels, which neither stage in shared memory nor
+    // synchronise per level.
+    const bool dmma = sizeof(T) == 8 && !knob_on(K_NO_DMMA);
     for (int l = levels - 1; l >= 0; --l) {
-        if (allow_fused && !knob_on(K_DISABLE_FUSED)) {
-            // group of levels l, l-1, ..., l-k+1 whose intermediate results are not trimmed -> one launch.
-            // float64: the synthesis cascade on the FP64 tensor cores (matrix_dmma.cuh), 2 levels per launch -- deeper
-            // cascades save HBM traffic but lose more to barriers and thin coarse levels.  float32: per-level kernels
-            // by default -- the scalar fused synthesis kernel reads shared memory with 2-way bank conflicts and
-            // synchronises once per level, the register-blocked per-level kernels do neither.
-            // WTB200_MATI_K sets the number of levels per launch for both.
-            const bool dmma = sizeof(T) == 8 && !knob_on(K_NO_DMMA);
-            int kmax = dmma ? 2 : 1;
+        if (dmma && allow_fused && !knob_on(K_DISABLE_FUSED)) {
+            // group of levels l, l-1, ..., l-k+1 whose intermediate results are not trimmed -> one launch, 2 levels
+            // per launch -- deeper cascades save HBM traffic but lose more to barriers and thin coarse levels.
+            // WTB200_MATI_K sets the number of levels per launch.
+            int kmax = 2;
             if (knob_is_set(K_MATI_K)) { const int v = (int)knob_val(K_MATI_K, 0); if (v >= 1 && v <= MATF_MAXK) kmax = v; }
             int k = 1;
-            const int64_t merge_n = dmma && !knob_is_set(K_MATI_K) ? knob_val(K_MATI_MERGE_N, 1024) : 0;
+            const int64_t merge_n = !knob_is_set(K_MATI_K) ? knob_val(K_MATI_MERGE_N, 1024) : 0;
             while (l - k >= 0 && next_len[l - k + 1] == n[l - k + 1] && n[l - k] == 2 * n[l - k + 1] &&
                    (k < kmax || (k < MATF_MAXK && n[l - k] <= merge_n)))
                 ++k;
@@ -677,22 +673,16 @@ static int matrix_inv_t(int levels, int L, const double* rlo, const double* rhi,
                 const int64_t dst_stride = last ? ys : (keep4 <= n[0] ? keep4 : keep0);
                 cudaError_t e = cudaSuccess;
                 bool launched = false;
-                if (keep0 == n[lf] || keep0 == n[lf] - 1) {
-                    if constexpr (sizeof(T) == 8) {
-                        if (dmma)
-                            launched = launch_mat_inv_dmma(L, k, n + lf, keep0, nbt + lf, nbb + lf, wt + lf, wb + lf,
-                                                           (const double* const*)(bptr + 4 * lf), (const double*)src, src_stride,
-                                                           hi_in + lf, hi_stride + lf, batch, (double*)dst, dst_stride, rlo, rhi,
-                                                           st, &e);
-                    }
-                    if (!launched && knob_is_set(K_MATI_K))
-                        launched = launch_mat_inv_fused<T>(L, k, n + lf, keep0, nbt + lf, nbb + lf, wt + lf, wb + lf,
-                                                           bptr + 4 * lf, src, src_stride, hi_in + lf, hi_stride + lf, batch,
-                                                           dst, dst_stride, rlo, rhi, st, &e);
+                if constexpr (sizeof(T) == 8) {
+                    if (keep0 == n[lf] || keep0 == n[lf] - 1)
+                        launched = launch_mat_inv_dmma(L, k, n + lf, keep0, nbt + lf, nbb + lf, wt + lf, wb + lf,
+                                                       (const double* const*)(bptr + 4 * lf), (const double*)src, src_stride,
+                                                       hi_in + lf, hi_stride + lf, batch, (double*)dst, dst_stride, rlo, rhi,
+                                                       st, &e);
                 }
                 if (launched) {
                     g_launches.fetch_add(1, std::memory_order_relaxed);
-                    if (e != cudaSuccess) return cuda_fail(e, "mat_inv_fused_kernel");
+                    if (e != cudaSuccess) return cuda_fail(e, "mat_inv_dmma_kernel");
                     src = dst; src_stride = dst_stride;
                     if (!last) pp ^= 1;
                     l = lf;

@@ -641,9 +641,9 @@ def test_calls_can_be_captured_in_a_cuda_graph():
     assert not torch.equal(leaves(eager)[0], want[0])
 
 
-def test_fused_matrix_synthesis_kernel_when_enabled(knob):
-    """WTB200_MATI_K >= 2 runs groups of synthesis levels as one kernel (intermediate approximations stay in
-    shared memory); it must agree with the oracle like the default per-level kernels."""
+def test_deep_matrix_synthesis_groups_on_the_fp64_tensor_cores(knob):
+    """WTB200_MATI_K=4 runs float64 MatrixWaverec as 4-level groups of the DMMA synthesis cascade (mat_inv_dmma_kernel,
+    intermediate approximations stay in shared memory) instead of the default 2; it must agree with the oracle."""
     knob("MATI_K", 4)
     g = torch.Generator().manual_seed(83)
     for wav, n, level in (("db2", 64, 3), ("db4", 256, 4), ("db6", 4096, 6), ("sym5", 1000, 5), ("haar", 48, 3),
@@ -655,14 +655,13 @@ def test_fused_matrix_synthesis_kernel_when_enabled(knob):
         assert_close_rel(got, want, scale=float(want.abs().max()), what=f"fused synthesis {wav} n={n} L{level}")
 
 
-@pytest.mark.parametrize("variant,nt", [(2, 128), (2, 256), (1, 128)])
-def test_matrix_analysis_on_the_fp64_tensor_cores(knob, variant, nt):
-    """float64 MatrixWavedec runs groups of levels as one DMMA cascade (matrix_dmma.cuh): the polyphase kernel (default)
-    or the streaming kernel (WTB200_MATF_VARIANT=1).  Both must agree with the oracle where its dense operators fit and
+@pytest.mark.parametrize("nt", [128, 256])
+def test_matrix_analysis_on_the_fp64_tensor_cores(knob, nt):
+    """float64 MatrixWavedec runs groups of levels as one DMMA cascade (mat_fwd_dmma2_kernel, the polyphase kernel in
+    matrix_dmma.cuh) with 128 or 256 threads per CTA.  It must agree with the oracle where its dense operators fit and
     with the per-level kernels (DISABLE_FUSED) everywhere, for every filter length, odd lengths and unaligned rows."""
-    knob("MATF_VARIANT", variant)
     knob("MATF_NT", nt)
-    g = torch.Generator().manual_seed(85 + variant)
+    g = torch.Generator().manual_seed(85 + 2)
     for wav, n, level, bs in (("haar", 64, 3, 5), ("db2", 96, None, 7), ("db3", 250, 4, 7), ("db4", 1000, None, 4),
                               ("sym5", 4096, 7, 7), ("db6", 5001, None, 3), ("db7", 20000, 5, 7), ("db8", 8192, None, 7),
                               ("db6", 65536, None, 7), ("db5", 40000, 3, 9)):
@@ -670,7 +669,7 @@ def test_matrix_analysis_on_the_fp64_tensor_cores(knob, variant, nt):
         got = wt.MatrixWavedec(wav, level)(x.to(DEV))
         with _native.knobs(DISABLE_FUSED=1):
             per_level = wt.MatrixWavedec(wav, level)(x.to(DEV))
-        tag = f"dmma analysis variant={variant} nt={nt} {wav} n={n} level={level}"
+        tag = f"dmma analysis nt={nt} {wav} n={n} level={level}"
         scale = max(float(t.abs().max()) for t in per_level)
         assert len(got) == len(per_level)
         for a, b in zip(got, per_level):
@@ -687,15 +686,11 @@ def test_matrix_analysis_on_the_fp64_tensor_cores(knob, variant, nt):
         assert_close_rel(a, b.contiguous(), scale=float(want[0].abs().max()), what="unaligned rows")
 
 
-@pytest.mark.parametrize("rows", [None, 0, -1, -3])
-def test_matrix_synthesis_on_the_fp64_tensor_cores(knob, rows):
-    """float64 MatrixWaverec runs groups of levels as one DMMA cascade (matrix_dmma.cuh): the row-streaming kernel
-    (TMA bulk staging, WTB200_MATI_ROWS < 0 forces that many rows per CTA) or, for unaligned / odd band lengths and MATI_ROWS=0, the
-    chunk-per-CTA kernel.  Both must agree with the oracle where the oracle's dense operators fit, with the per-level
-    kernels (NO_DMMA) everywhere, and invert MatrixWavedec."""
-    if rows is not None:
-        knob("MATI_ROWS", rows)
-    g = torch.Generator().manual_seed(84 + abs(rows or 0))
+def test_matrix_synthesis_on_the_fp64_tensor_cores():
+    """float64 MatrixWaverec runs groups of levels as one DMMA cascade (mat_inv_dmma_kernel in matrix_dmma.cuh, one
+    chunk of the finest output per CTA).  It must agree with the oracle where the oracle's dense operators fit, with
+    the per-level kernels (NO_DMMA) everywhere, and invert MatrixWavedec, on aligned and unaligned rows."""
+    g = torch.Generator().manual_seed(84)
     for wav, n, level, bs in (("haar", 64, 3, 5), ("db2", 96, None, 7), ("db3", 250, 4, 7), ("db4", 1000, None, 4),
                               ("sym5", 4096, 7, 7), ("db6", 5001, None, 3), ("db7", 20000, 5, 7), ("db8", 8192, None, 7),
                               ("db6", 65536, None, 7), ("db4", 65536, 2, 5)):
@@ -704,13 +699,13 @@ def test_matrix_synthesis_on_the_fp64_tensor_cores(knob, rows):
         got = wt.MatrixWaverec(wav)(co)
         with _native.knobs(NO_DMMA=1):
             per_level = wt.MatrixWaverec(wav)(co)
-        tag = f"dmma synthesis rows={rows} {wav} n={n} level={level}"
+        tag = f"dmma synthesis {wav} n={n} level={level}"
         assert_close_rel(got, per_level, scale=float(per_level.abs().max()), what=tag + " vs per-level kernels")
         assert float((got[..., :n].cpu() - x).abs().max()) < 1e-9, tag + " round trip"
         if n <= 4096:
             want = P.MatrixWaverec(wav)([t.cpu() for t in co])
             assert_close_rel(got, want.contiguous(), scale=float(want.abs().max()), what=tag + " vs oracle")
-    # strided views of a packed buffer (rows not 16-byte aligned -> chunk-per-CTA kernel with 8-byte copies)
+    # strided views of a packed buffer (rows not 16-byte aligned -> 8-byte copies)
     x = torch.randn((6, 1024), generator=g, dtype=torch.float64)
     co = wt.MatrixWavedec("db4", 4)(x.to(DEV))
     odd = [torch.empty(6, t.shape[-1] + 1, device=DEV, dtype=torch.float64)[:, 1:].copy_(t) for t in co]

@@ -75,18 +75,39 @@ def test_bad_arguments_are_rejected_without_a_gpu():
         _native.check(rc, "wt_dwt_fwd")
 
 
-def test_knob_registry_round_trips_and_rejects_unknown_names():
-    """The tuning / test switches (csrc/knobs.cuh) are process state of the library, set through the C ABI: every
-    name the source lists is accepted, set / get / unset round-trip, negative values survive (MATI_ROWS < 0 is
-    meaningful), unknown names fail with WT_EINVAL instead of being silently ignored."""
+KNOB_NAMES = (
+    "DISABLE_FUSED", "NO_FFMA2", "CHUNK", "STREAMS", "FWD3D_TILE", "CONVF_CHUNK", "CONVF_K", "MATF_CHUNK",
+    "MATI_CHUNK", "MATF_K", "MATI_K", "MATI_NT", "MATI_MINCTAS", "MATI_MERGE_N", "MATF_KCOARSE", "NO_WPAIR",
+    "WPAIR_SEG", "WPAIR_MIN", "WPAIR_DEEP", "NO_AUX_STREAM", "WPAIR_VAR", "WPAIR", "MATF_NT", "MATF_MINB", "MATF_CPC",
+    "NO_DMMA", "FUSE2",
+)
+# switches of matrix-FWT kernels that have been removed: unknown names now
+RETIRED_KNOB_NAMES = ("MATF_VARIANT", "DMMA_PERM", "MATF_MINCTAS", "MATI_ROWS")
+
+
+def test_knob_registry_lists_exactly_the_live_switches_and_rejects_retired_ones():
+    """The tuning / test switches (csrc/knobs.cuh) are process state of the library, set through the C ABI: exactly
+    the names listed here are accepted, set / get / unset round-trip, negative values survive, unknown and retired
+    names fail with WT_EINVAL instead of being silently ignored."""
     from pytorch_wavelet_toolbox_b200 import _native
 
     text = (ROOT / "pytorch_wavelet_toolbox_b200" / "csrc" / "knobs.cuh").read_text()
     body = text[text.index("#define WTB_KNOB_LIST(X)"):text.index("enum KnobId")]
     names = re.findall(r"X\(([A-Z0-9_]+)\)", body)
-    assert len(names) >= 30 and len(names) == len(set(names))
-    for must in ("NO_DMMA", "MATF_VARIANT", "MATI_ROWS", "MATI_K", "MATF_K", "WPAIR", "DISABLE_FUSED"):
+    assert len(KNOB_NAMES) == 27
+    assert tuple(names) == KNOB_NAMES
+    for must in ("NO_DMMA", "MATI_K", "MATF_K", "WPAIR", "DISABLE_FUSED"):
         assert must in names
+    lib = _native.load()
+    for name in RETIRED_KNOB_NAMES:
+        assert name not in names
+        value = ctypes.c_longlong(0)
+        assert lib.wt_set_knob(name.encode(), 1) == -1 and b"unknown knob" in lib.wt_last_error()  # WT_EINVAL
+        assert lib.wt_get_knob(name.encode(), ctypes.byref(value)) == -1
+        with pytest.raises(_native.NativeError):
+            _native.set_knob(name, 1)
+        with pytest.raises(_native.NativeError):
+            _native.get_knob(name)
     for name in names:
         before = _native.get_knob(name)
         with _native.knobs(**{name: -3}):
