@@ -232,6 +232,33 @@ int wt_matrix_axis_inv(int dtype, int filt_len, const double* rec_lo, const doub
 int wt_tap_corr(int dtype, int filt_len, const void* coeff_lo, const void* coeff_hi, int64_t coeff_stride,
                 const void* sig, int64_t sig_stride, int64_t rows, int64_t m, int64_t n, double* out, void* stream);
 
+/* Stationary wavelet transform (ptwt.swt / ptwt.iswt), periodic extension, 1-D along contiguous rows of n samples.
+ *   wt_swt_fwd  <- the level loop of swt,  src/ptwt/stationary_transform.py:96-106
+ *                  (_circular_pad -> conv1d(dilation 2^(j-1)) -> split)
+ *   wt_swt_inv  <- the level loop of iswt, src/ptwt/stationary_transform.py:139-151
+ *                  (stack -> _circular_pad -> conv_transpose1d(dilation 2^(j-1), groups 2) -> mean)
+ * Taps are host doubles in WINDOW order (not PyWavelets order), with any scale folded in; hl = L/2 - 1, L even:
+ *   analysis   c_lo/hi[i] = sum_m f_lo/hi[m] a[(i + d (m - hl)) mod n]        swt: f = dec[::-1]
+ *   synthesis  y[i] = sum_m g_lo[m] a[(i + d (hl - m)) mod n] + g_hi[m] c[same]  iswt: g = 0.5 * rec
+ * The two forms are adjoint: analysis with f = 0.5 rec is the gradient of synthesis, synthesis with g = dec[::-1]
+ * the gradient of analysis.
+ * wt_swt_fwd writes [cA_J, cD_J, ..., cD_1] as bands of `out` (band b at out + b * out_band_stride, batch item at
+ * + item * out_batch_stride); wt_swt_inv reads cA_J from `approx` and cD_j from details + (levels - j) * band stride.
+ * tables: NULL, or `levels` device pointers (level j at [j-1]); a non-NULL entry replaces the periodic index of that
+ * level by a CSR table: int32 rowptr[n + 1], then from int32 offset 2 * ((n + 2) / 2) the (source index, tap) int32
+ * pairs of every output (the reference's _circular_pad when a pad exceeds n, or its transpose for the adjoint).
+ * workspace: wt_swt_workspace_bytes() bytes (0 when the levels run in one launch). */
+size_t wt_swt_workspace_bytes(int dtype, int levels, int filt_len, int64_t batch, int64_t n,
+                              const void* const* tables, int inverse);
+int wt_swt_fwd(int dtype, int levels, int filt_len, const double* f_lo, const double* f_hi, const void* x,
+               int64_t batch, int64_t n, int64_t x_batch_stride, void* out, int64_t out_batch_stride,
+               int64_t out_band_stride, const void* const* tables, void* workspace, size_t workspace_bytes,
+               void* stream);
+int wt_swt_inv(int dtype, int levels, int filt_len, const double* g_lo, const double* g_hi, const void* approx,
+               int64_t approx_batch_stride, const void* details, int64_t details_batch_stride,
+               int64_t details_band_stride, int64_t batch, int64_t n, void* y, int64_t y_batch_stride,
+               const void* const* tables, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Counters for bench.py's gpu_launches claim: kernels launched by this library on this
  * process since the last reset. */
 uint64_t wt_launch_count(void);

@@ -26,6 +26,7 @@ from .matrix_fwt import MatrixWavedec, MatrixWaverec, construct_boundary_a, cons
 from .matrix_fwt_nd import MatrixWavedec2, MatrixWavedec3, MatrixWaverec2, MatrixWaverec3
 from .separable import fswavedec2, fswavedec3, fswaverec2, fswaverec3
 from .packets import WaveletPacket, WaveletPacket2D
+from .stationary import iswt, swt
 
 __version__ = "0.1.0"
 
@@ -37,6 +38,7 @@ NEXT_ROW_NAMES = (
     "fswavedec2", "fswavedec3", "fswaverec2", "fswaverec3",
     "MatrixWavedec2", "MatrixWaverec2", "MatrixWavedec3", "MatrixWaverec3",  # separable mode only
     "WaveletPacket", "WaveletPacket2D",                                      # level-wise batched node expansion
+    "swt", "iswt",                                                           # stationary transform, csrc/swt.cuh
 )
 
 __all__ = list(HOT_PATH_NAMES) + list(NEXT_ROW_NAMES) + [

@@ -20,6 +20,7 @@
 #include "matrix_dmma.cuh"
 #include "axis1d_fused.cuh"
 #include "tap_grad.cuh"
+#include "swt.cuh"
 
 namespace wtb {
 
@@ -815,9 +816,156 @@ static int matrix_axis_check(int dtype, int filt_len, const double* lo, const do
     return 0;
 }
 
+// ---- stationary transform -------------------------------------------------------------------------------------
+static int swt_check(int dtype, int levels, int filt_len, const double* t0, const double* t1, int64_t batch, int64_t n) {
+    if (dtype != WT_F32 && dtype != WT_F64) return fail(WT_EINVAL, "dtype must be WT_F32 or WT_F64");
+    if (filt_len < 2 || filt_len > WT_MAX_FILT_LEN || (filt_len & 1))
+        return fail(WT_EUNSUPPORTED, "filter length %d (even, 2..%d)", filt_len, WT_MAX_FILT_LEN);
+    if (levels < 0 || levels > 40) return fail(WT_EINVAL, "levels %d", levels);
+    if (batch < 0 || n < 1) return fail(WT_ESHAPE, "batch %lld, n %lld", (long long)batch, (long long)n);
+    if (!t0 || !t1) return fail(WT_EINVAL, "NULL filter");
+    return 0;
+}
+
+// Which buffer receives the approximation leaving step s of ns (in execution order): the last step writes the
+// final one, the others alternate between the workspace and that final buffer, so no step reads what it writes.
+static inline bool swt_to_workspace(int s, int ns) { return ((ns - 1 - s) & 1) != 0; }
+
+template <typename T>
+static int swt_fwd_t(int levels, int L, const double* f_lo, const double* f_hi, const T* x, int64_t batch, int64_t n,
+                     int64_t xbs, T* out, int64_t obs, int64_t band, const void* const* tables, T* ws, size_t ws_bytes,
+                     cudaStream_t st) {
+    SwtStep steps[64];
+    const int ns = swt_plan(sizeof(T), false, levels, L, n, tables, steps);
+    if (ns > 1 && ws_bytes < (size_t)(batch * n) * sizeof(T)) return fail(WT_EWORKSPACE, "swt workspace too small");
+    const T* in = x;
+    int64_t in_bs = xbs;
+    for (int s = 0; s < ns; ++s) {
+        const SwtStep& S = steps[s];
+        const bool to_ws = swt_to_workspace(s, ns);
+        T* a_out = to_ws ? ws : out;
+        const int64_t a_bs = to_ws ? n : obs;
+        cudaError_t e;
+        if (S.tiled) {
+            SwtTileParams<T> p;
+            memset(&p, 0, sizeof(p));
+            p.a = in; p.a_bs = in_bs; p.out = a_out; p.out_bs = a_bs;
+            for (int k = 0; k < S.K; ++k) p.det[k] = out + (int64_t)(levels + 1 - (S.j0 + k)) * band;
+            p.det_bs = obs; p.batch = batch;
+            p.D = S.D; p.M = n / S.D; p.d0 = S.d0; p.C = S.C;
+            p.K = S.K; p.R = S.R; p.lgR = S.lgR; p.L = L;
+            for (int m = 0; m < L; ++m) { p.f0[m] = (T)f_lo[m]; p.f1[m] = (T)f_hi[m]; }
+            e = swt_run_tile<T>(false, p, st);
+        } else {
+            SwtLevelParams<T> p;
+            memset(&p, 0, sizeof(p));
+            p.a0 = in; p.a0_bs = in_bs;
+            p.o0 = a_out; p.o0_bs = a_bs;
+            p.o1 = out + (int64_t)(levels + 1 - S.j0) * band; p.o1_bs = obs;
+            p.batch = batch; p.n = n; p.d = int64_t(1) << (S.j0 - 1); p.L = L;
+            p.tab = tables ? (const int32_t*)tables[S.j0 - 1] : nullptr;
+            for (int m = 0; m < L; ++m) { p.f0[m] = (T)f_lo[m]; p.f1[m] = (T)f_hi[m]; }
+            e = swt_run_level<T>(false, p, st);
+        }
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if (e != cudaSuccess) return cuda_fail(e, S.tiled ? "swt_fwd_kernel" : "swt_level_kernel");
+        in = a_out;
+        in_bs = a_bs;
+    }
+    return 0;
+}
+
+template <typename T>
+static int swt_inv_t(int levels, int L, const double* g_lo, const double* g_hi, const T* approx, int64_t abs_,
+                     const T* det, int64_t dbs, int64_t band, int64_t batch, int64_t n, T* y, int64_t ybs,
+                     const void* const* tables, T* ws, size_t ws_bytes, cudaStream_t st) {
+    SwtStep steps[64];
+    const int ns = swt_plan(sizeof(T), true, levels, L, n, tables, steps);
+    if (ns > 1 && ws_bytes < (size_t)(batch * n) * sizeof(T)) return fail(WT_EWORKSPACE, "iswt workspace too small");
+    const T* in = approx;
+    int64_t in_bs = abs_;
+    for (int s = 0; s < ns; ++s) {                       // coarsest group first
+        const SwtStep& S = steps[ns - 1 - s];
+        const bool to_ws = swt_to_workspace(s, ns);
+        T* a_out = to_ws ? ws : y;
+        const int64_t a_bs = to_ws ? n : ybs;
+        cudaError_t e;
+        if (S.tiled) {
+            SwtTileParams<T> p;
+            memset(&p, 0, sizeof(p));
+            p.a = in; p.a_bs = in_bs; p.out = a_out; p.out_bs = a_bs;
+            for (int k = 0; k < S.K; ++k) p.det[k] = const_cast<T*>(det) + (int64_t)(levels - (S.j0 + k)) * band;
+            p.det_bs = dbs; p.batch = batch;
+            p.D = S.D; p.M = n / S.D; p.d0 = S.d0; p.C = S.C;
+            p.K = S.K; p.R = S.R; p.lgR = S.lgR; p.L = L;
+            for (int m = 0; m < L; ++m) { p.f0[m] = (T)g_lo[m]; p.f1[m] = (T)g_hi[m]; }
+            e = swt_run_tile<T>(true, p, st);
+        } else {
+            SwtLevelParams<T> p;
+            memset(&p, 0, sizeof(p));
+            p.a0 = in; p.a0_bs = in_bs;
+            p.a1 = det + (int64_t)(levels - S.j0) * band; p.a1_bs = dbs;
+            p.o0 = a_out; p.o0_bs = a_bs;
+            p.batch = batch; p.n = n; p.d = int64_t(1) << (S.j0 - 1); p.L = L;
+            p.tab = tables ? (const int32_t*)tables[S.j0 - 1] : nullptr;
+            for (int m = 0; m < L; ++m) { p.f0[m] = (T)g_lo[m]; p.f1[m] = (T)g_hi[m]; }
+            e = swt_run_level<T>(true, p, st);
+        }
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if (e != cudaSuccess) return cuda_fail(e, S.tiled ? "swt_inv_kernel" : "swt_level_kernel");
+        in = a_out;
+        in_bs = a_bs;
+    }
+    return 0;
+}
+
 extern "C" {
 
 int wt_version(void) { return WT_VERSION; }
+
+size_t wt_swt_workspace_bytes(int dtype, int levels, int filt_len, int64_t batch, int64_t n,
+                              const void* const* tables, int inverse) {
+    if ((dtype != WT_F32 && dtype != WT_F64) || levels < 1 || levels > 40 || filt_len < 2 ||
+        filt_len > WT_MAX_FILT_LEN || (filt_len & 1) || batch < 1 || n < 1)
+        return 0;
+    const int es = dtype == WT_F64 ? 8 : 4;
+    SwtStep steps[64];
+    return swt_plan(es, inverse != 0, levels, filt_len, n, tables, steps) > 1 ? (size_t)(batch * n) * es : 0;
+}
+
+int wt_swt_fwd(int dtype, int levels, int filt_len, const double* f_lo, const double* f_hi, const void* x,
+               int64_t batch, int64_t n, int64_t x_batch_stride, void* out, int64_t out_batch_stride,
+               int64_t out_band_stride, const void* const* tables, void* workspace, size_t workspace_bytes,
+               void* stream) {
+    int rc = swt_check(dtype, levels, filt_len, f_lo, f_hi, batch, n);
+    if (rc) return rc;
+    if (levels == 0 || batch == 0) return 0;
+    if (!x || !out) return fail(WT_EINVAL, "NULL argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32)
+        return swt_fwd_t<float>(levels, filt_len, f_lo, f_hi, (const float*)x, batch, n, x_batch_stride, (float*)out,
+                                out_batch_stride, out_band_stride, tables, (float*)workspace, workspace_bytes, st);
+    return swt_fwd_t<double>(levels, filt_len, f_lo, f_hi, (const double*)x, batch, n, x_batch_stride, (double*)out,
+                             out_batch_stride, out_band_stride, tables, (double*)workspace, workspace_bytes, st);
+}
+
+int wt_swt_inv(int dtype, int levels, int filt_len, const double* g_lo, const double* g_hi, const void* approx,
+               int64_t approx_batch_stride, const void* details, int64_t details_batch_stride,
+               int64_t details_band_stride, int64_t batch, int64_t n, void* y, int64_t y_batch_stride,
+               const void* const* tables, void* workspace, size_t workspace_bytes, void* stream) {
+    int rc = swt_check(dtype, levels, filt_len, g_lo, g_hi, batch, n);
+    if (rc) return rc;
+    if (levels == 0 || batch == 0) return 0;
+    if (!approx || !details || !y) return fail(WT_EINVAL, "NULL argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32)
+        return swt_inv_t<float>(levels, filt_len, g_lo, g_hi, (const float*)approx, approx_batch_stride,
+                                (const float*)details, details_batch_stride, details_band_stride, batch, n, (float*)y,
+                                y_batch_stride, tables, (float*)workspace, workspace_bytes, st);
+    return swt_inv_t<double>(levels, filt_len, g_lo, g_hi, (const double*)approx, approx_batch_stride,
+                             (const double*)details, details_batch_stride, details_band_stride, batch, n, (double*)y,
+                             y_batch_stride, tables, (double*)workspace, workspace_bytes, st);
+}
 
 const char* wt_last_error(void) { return g_err; }
 
