@@ -259,6 +259,34 @@ int wt_swt_inv(int dtype, int levels, int filt_len, const double* g_lo, const do
                int64_t details_band_stride, int64_t batch, int64_t n, void* y, int64_t y_batch_stride,
                const void* const* tables, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Continuous wavelet transform (ptwt.cwt), src/ptwt/continuous_transform.py:103-137 (per scale: FFT of the
+ * filter and the data, product, inverse FFT, diff, crop; then stack), as uniformly partitioned overlap-save in
+ * float64 (csrc/cwt.cuh).  Hop H = 2^(fft_log2 - 1), FFT size F = 2H, fft_log2 in 6..12; nb = ceil(n / H).
+ * A channel is one complex-wavelet scale (complex_out != 0) or a pair of real-wavelet scales whose taps are packed
+ * as real + i * imaginary (complex_out == 0).  Channel c's FIR is  y_c[t] = sum_j taps_c[j] x[t + d_c H + e_c - j]
+ * (0 <= e_c < H); its taps are cut into P_c parts of H.
+ *   wt_cwt_filter_spectra: spectra[r] = FFT(taps[r] zero-padded to F) / F, in bit-reversed bin order, for `parts`
+ *                          rows of H complex128 taps (all device buffers; twiddles[k] = exp(-2 pi i k / F), k < F / 2,
+ *                          complex128).
+ *   wt_cwt_fwd: meta = device int32 [channels][6] = {first part row, P_c, d_c, scale s1, scale s2 or -1, e_c};
+ *               x [batch] rows of n samples (WT_F32/WT_F64, unit stride) -> float64 (complex_out == 0: s1 gets the
+ *               real part, s2 the imaginary part) or complex128 coefficients at
+ *               out + s * out_scale_stride + item * out_batch_stride + t (strides in elements of the output type).
+ *   wt_cwt_adj: the adjoint, gx[item][m] = Re sum_c sum_t conj(taps_c[t + d_c H + e_c - m]) gy_c[t], gy laid out like
+ *               wt_cwt_fwd's output, gx in `dtype`.
+ * workspace: wt_cwt_workspace_bytes() bytes (the batch runs in chunks that fit a fixed budget, two launches each). */
+size_t wt_cwt_workspace_bytes(int fft_log2, int64_t batch, int64_t n, int64_t channels, int adjoint);
+int wt_cwt_filter_spectra(int fft_log2, int64_t parts, const void* taps, const void* twiddles, void* spectra,
+                          void* stream);
+int wt_cwt_fwd(int dtype, int fft_log2, int64_t channels, const int32_t* meta, const void* spectra,
+               const void* twiddles, int complex_out, const void* x, int64_t batch, int64_t n, int64_t x_batch_stride,
+               void* out, int64_t out_scale_stride, int64_t out_batch_stride, void* workspace, size_t workspace_bytes,
+               void* stream);
+int wt_cwt_adj(int dtype, int fft_log2, int64_t channels, const int32_t* meta, const void* spectra,
+               const void* twiddles, int complex_out, const void* gy, int64_t out_scale_stride,
+               int64_t out_batch_stride, int64_t batch, int64_t n, void* gx, int64_t gx_batch_stride,
+               void* workspace, size_t workspace_bytes, void* stream);
+
 /* Counters for bench.py's gpu_launches claim: kernels launched by this library on this
  * process since the last reset. */
 uint64_t wt_launch_count(void);

@@ -27,6 +27,7 @@ from .matrix_fwt_nd import MatrixWavedec2, MatrixWavedec3, MatrixWaverec2, Matri
 from .separable import fswavedec2, fswavedec3, fswaverec2, fswaverec3
 from .packets import WaveletPacket, WaveletPacket2D
 from .stationary import iswt, swt
+from .continuous import cwt
 
 __version__ = "0.1.0"
 
@@ -39,6 +40,7 @@ NEXT_ROW_NAMES = (
     "MatrixWavedec2", "MatrixWaverec2", "MatrixWavedec3", "MatrixWaverec3",  # separable mode only
     "WaveletPacket", "WaveletPacket2D",                                      # level-wise batched node expansion
     "swt", "iswt",                                                           # stationary transform, csrc/swt.cuh
+    "cwt",                                                                   # continuous transform, csrc/cwt.cuh
 )
 
 __all__ = list(HOT_PATH_NAMES) + list(NEXT_ROW_NAMES) + [

@@ -21,6 +21,7 @@
 #include "axis1d_fused.cuh"
 #include "tap_grad.cuh"
 #include "swt.cuh"
+#include "cwt.cuh"
 
 namespace wtb {
 
@@ -919,9 +920,158 @@ static int swt_inv_t(int levels, int L, const double* g_lo, const double* g_hi, 
     return 0;
 }
 
+// ---- continuous transform --------------------------------------------------------------------------------------
+// The batch runs in chunks of signals whose spectra fit CWT_WS_BUDGET; one chunk costs two launches.
+constexpr size_t CWT_WS_BUDGET = size_t(1) << 29;
+
+static int64_t cwt_blocks(int64_t n, int lg) { return (n + (int64_t(1) << (lg - 1)) - 1) >> (lg - 1); }
+
+static size_t cwt_signal_bytes(int lg, int64_t n, int64_t channels, bool adjoint) {
+    const int64_t nb = cwt_blocks(n, lg);
+    return (size_t)((adjoint ? channels : 1) * (nb + 1) << lg) * sizeof(double2);
+}
+
+static int64_t cwt_chunk(int lg, int64_t batch, int64_t n, int64_t channels, bool adjoint) {
+    const size_t per = cwt_signal_bytes(lg, n, channels, adjoint);
+    int64_t c = (int64_t)std::max<size_t>(1, CWT_WS_BUDGET / per);
+    return std::min<int64_t>(std::min<int64_t>(c, batch), 65535);
+}
+
+static int cwt_check(int lg, int64_t channels, int64_t batch, int64_t n) {
+    if (lg < CWT_MIN_LOG2 || lg > CWT_MAX_LOG2)
+        return fail(WT_EUNSUPPORTED, "cwt FFT size 2^%d (2^%d..2^%d)", lg, CWT_MIN_LOG2, CWT_MAX_LOG2);
+    if (channels < 1 || batch < 0 || n < 1)
+        return fail(WT_ESHAPE, "cwt channels %lld, batch %lld, n %lld", (long long)channels, (long long)batch,
+                    (long long)n);
+    if ((cwt_blocks(n, lg) + 1) * channels > INT32_MAX)
+        return fail(WT_ESHAPE, "cwt grid too large");
+    return 0;
+}
+
+template <typename K>
+static cudaError_t cwt_prepare(K kern) { return ensure_dyn_smem(kern, sizeof(double2) << CWT_MAX_LOG2); }
+
+template <typename T>
+static int cwt_fwd_t(CwtParams p, const T* x, int64_t batch, int64_t xbs, bool cplx, double2* ws, size_t ws_bytes,
+                     cudaStream_t st) {
+    const int64_t chunk = cwt_chunk(p.lg, batch, p.n, p.channels, false);
+    if (ws_bytes < (size_t)chunk * cwt_signal_bytes(p.lg, p.n, p.channels, false))
+        return fail(WT_EWORKSPACE, "cwt workspace too small");
+    const size_t smem = sizeof(double2) << p.lg;
+    cudaError_t e = cwt_prepare(cwt_data_spectra_kernel<T>);
+    if (e == cudaSuccess) e = cwt_prepare(cplx ? cwt_main_kernel<true> : cwt_main_kernel<false>);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(cwt)");
+    p.X = ws;
+    for (int64_t s0 = 0; s0 < batch; s0 += chunk) {
+        const int64_t cs = std::min(chunk, batch - s0);
+        cwt_data_spectra_kernel<T><<<dim3((unsigned)p.nq, (unsigned)cs), CWT_THREADS, smem, st>>>(
+            x + s0 * xbs, xbs, p.n, p.nq, p.lg, p.tw, ws);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "cwt_data_spectra_kernel");
+        p.sig0 = s0;
+        const dim3 grid((unsigned)(p.nq * p.channels), 1, (unsigned)cs);
+        if (cplx) cwt_main_kernel<true><<<grid, CWT_THREADS, smem, st>>>(p);
+        else cwt_main_kernel<false><<<grid, CWT_THREADS, smem, st>>>(p);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "cwt_main_kernel");
+    }
+    return 0;
+}
+
+template <typename T>
+static int cwt_adj_t(CwtParams p, int64_t batch, bool cplx, double2* ws, size_t ws_bytes, cudaStream_t st) {
+    const int64_t chunk = cwt_chunk(p.lg, batch, p.n, p.channels, true);
+    if (ws_bytes < (size_t)chunk * cwt_signal_bytes(p.lg, p.n, p.channels, true))
+        return fail(WT_EWORKSPACE, "cwt adjoint workspace too small");
+    const size_t smem = sizeof(double2) << p.lg;
+    cudaError_t e = cwt_prepare(cplx ? cwt_adj_spectra_kernel<true> : cwt_adj_spectra_kernel<false>);
+    if (e == cudaSuccess) e = cwt_prepare(cwt_adj_main_kernel<T>);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(cwt adjoint)");
+    p.X = ws;
+    for (int64_t s0 = 0; s0 < batch; s0 += chunk) {
+        const int64_t cs = std::min(chunk, batch - s0);
+        p.sig0 = s0;
+        const dim3 g1((unsigned)(p.nq * p.channels), (unsigned)cs);
+        if (cplx) cwt_adj_spectra_kernel<true><<<g1, CWT_THREADS, smem, st>>>(p, ws);
+        else cwt_adj_spectra_kernel<false><<<g1, CWT_THREADS, smem, st>>>(p, ws);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "cwt_adj_spectra_kernel");
+        cwt_adj_main_kernel<T><<<dim3((unsigned)p.nb, (unsigned)cs), CWT_THREADS, smem, st>>>(p);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "cwt_adj_main_kernel");
+    }
+    return 0;
+}
+
+static CwtParams cwt_params(int lg, int64_t channels, const int32_t* meta, const void* spectra, const void* twiddles,
+                            int64_t n, int64_t out_scale_stride, int64_t out_batch_stride) {
+    CwtParams p;
+    memset(&p, 0, sizeof(p));
+    p.meta = meta; p.spec = (const double2*)spectra; p.tw = (const double2*)twiddles;
+    p.n = n; p.nb = cwt_blocks(n, lg); p.nq = p.nb + 1; p.channels = channels;
+    p.o_scale = out_scale_stride; p.o_batch = out_batch_stride; p.lg = lg;
+    return p;
+}
+
 extern "C" {
 
 int wt_version(void) { return WT_VERSION; }
+
+size_t wt_cwt_workspace_bytes(int fft_log2, int64_t batch, int64_t n, int64_t channels, int adjoint) {
+    if (cwt_check(fft_log2, channels, batch, n) || batch < 1) return 0;
+    return (size_t)cwt_chunk(fft_log2, batch, n, channels, adjoint != 0) *
+           cwt_signal_bytes(fft_log2, n, channels, adjoint != 0);
+}
+
+int wt_cwt_filter_spectra(int fft_log2, int64_t parts, const void* taps, const void* twiddles, void* spectra,
+                          void* stream) {
+    if (fft_log2 < CWT_MIN_LOG2 || fft_log2 > CWT_MAX_LOG2) return fail(WT_EUNSUPPORTED, "cwt FFT size 2^%d", fft_log2);
+    if (parts < 0 || parts > INT32_MAX) return fail(WT_ESHAPE, "cwt filter parts %lld", (long long)parts);
+    if (parts == 0) return 0;
+    if (!taps || !twiddles || !spectra) return fail(WT_EINVAL, "NULL argument");
+    cudaError_t e = cwt_prepare(cwt_filter_spectra_kernel);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(cwt_filter_spectra_kernel)");
+    cwt_filter_spectra_kernel<<<(unsigned)parts, CWT_THREADS, sizeof(double2) << fft_log2, (cudaStream_t)stream>>>(
+        (const double2*)taps, (const double2*)twiddles, (double2*)spectra, fft_log2);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "cwt_filter_spectra_kernel");
+    return 0;
+}
+
+int wt_cwt_fwd(int dtype, int fft_log2, int64_t channels, const int32_t* meta, const void* spectra,
+               const void* twiddles, int complex_out, const void* x, int64_t batch, int64_t n, int64_t x_batch_stride,
+               void* out, int64_t out_scale_stride, int64_t out_batch_stride, void* workspace, size_t workspace_bytes,
+               void* stream) {
+    if (dtype != WT_F32 && dtype != WT_F64) return fail(WT_EINVAL, "dtype must be WT_F32 or WT_F64");
+    int rc = cwt_check(fft_log2, channels, batch, n);
+    if (rc) return rc;
+    if (batch == 0) return 0;
+    if (!meta || !spectra || !twiddles || !x || !out || !workspace) return fail(WT_EINVAL, "NULL argument");
+    CwtParams p = cwt_params(fft_log2, channels, meta, spectra, twiddles, n, out_scale_stride, out_batch_stride);
+    p.out = out;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32)
+        return cwt_fwd_t<float>(p, (const float*)x, batch, x_batch_stride, complex_out != 0, (double2*)workspace,
+                                workspace_bytes, st);
+    return cwt_fwd_t<double>(p, (const double*)x, batch, x_batch_stride, complex_out != 0, (double2*)workspace,
+                             workspace_bytes, st);
+}
+
+int wt_cwt_adj(int dtype, int fft_log2, int64_t channels, const int32_t* meta, const void* spectra,
+               const void* twiddles, int complex_out, const void* gy, int64_t out_scale_stride,
+               int64_t out_batch_stride, int64_t batch, int64_t n, void* gx, int64_t gx_batch_stride,
+               void* workspace, size_t workspace_bytes, void* stream) {
+    if (dtype != WT_F32 && dtype != WT_F64) return fail(WT_EINVAL, "dtype must be WT_F32 or WT_F64");
+    int rc = cwt_check(fft_log2, channels, batch, n);
+    if (rc) return rc;
+    if (batch == 0) return 0;
+    if (!meta || !spectra || !twiddles || !gy || !gx || !workspace) return fail(WT_EINVAL, "NULL argument");
+    CwtParams p = cwt_params(fft_log2, channels, meta, spectra, twiddles, n, out_scale_stride, out_batch_stride);
+    p.gy = gy; p.out = gx; p.gx_bs = gx_batch_stride;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32) return cwt_adj_t<float>(p, batch, complex_out != 0, (double2*)workspace, workspace_bytes, st);
+    return cwt_adj_t<double>(p, batch, complex_out != 0, (double2*)workspace, workspace_bytes, st);
+}
 
 size_t wt_swt_workspace_bytes(int dtype, int levels, int filt_len, int64_t batch, int64_t n,
                               const void* const* tables, int inverse) {
