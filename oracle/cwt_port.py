@@ -35,7 +35,11 @@ def _samples(wavelet: Any, precision: int, device: torch.device):
     return integral.to(device), grid.to(torch.float64)
 
 
-def cwt(data: torch.Tensor, scales: Any, wavelet: Any, sampling_period: float = 1.0, precision: int = 12):
+def cwt(data: torch.Tensor, scales: Any, wavelet: Any, sampling_period: float = 1.0, precision: int = 12,
+        index_dtype: Any = None):
+    """``index_dtype``: the dtype in which the sample positions of the scaled wavelet are computed (default: the
+    data's, as the reference does).  A float32 transform picks its taps in float32; checking it with float64
+    arithmetic needs the same taps."""
     wav = as_continuous_wavelet(wavelet)
     if isinstance(scales, torch.Tensor):
         scales = scales.cpu().numpy()
@@ -49,7 +53,7 @@ def cwt(data: torch.Tensor, scales: Any, wavelet: Any, sampling_period: float = 
     for s in scales:
         # on the CPU whatever the data's device: CUDA divides a float32 tensor by a scalar as a multiplication by the
         # reciprocal, which picks other taps at some scales than the reference's CPU tables (the fixtures) do
-        pos = torch.arange(float(s) * (hi - lo) + 1, dtype=data.dtype) / (float(s) * dx)
+        pos = torch.arange(float(s) * (hi - lo) + 1, dtype=index_dtype or data.dtype) / (float(s) * dx)
         pos = torch.floor(pos).long()
         pos = pos[pos < int_psi.shape[0]]
         taps = torch.flip(int_psi.cpu()[pos], (0,)).to(data.device)
