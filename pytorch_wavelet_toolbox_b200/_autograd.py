@@ -24,6 +24,14 @@ the filters enter the two Functions as tensor inputs.  Per axis the tap gradient
 ``sum_i c[i] * s[2 i + t + 2 - L]`` of the band gradients -- carried through the ADJOINT of the other axes' passes
 with the same single-axis kernels -- with the level input (analysis), or of the bands -- carried through the other
 axes' synthesis passes -- with the output gradient (synthesis); ``wt_tap_corr`` (csrc/tap_grad.cuh) evaluates it.
+
+Higher-order gradients (``create_graph=True``: gradient penalties, Hessian-vector products): the three Functions are
+each other's adjoints, so when a backward pass runs in grad mode it computes the same quantities through the other
+Function's ``apply`` with the flipped tap TENSORS (saved by every Function) instead of a raw launch, and the tap
+correlation runs through ``TapCorrelation``, whose backward is one synthesis pass (signal side) and one zero-extension
+analysis pass (coefficient side) with the cotangent as taps.  Every node of such a graph is again one of these four
+Functions or differentiable index / pad / slice glue, so gradients of any order reach the data and the filters.  With
+``create_graph=False`` the backward passes launch the kernels directly, as they always have.
 """
 from __future__ import annotations
 
@@ -150,17 +158,31 @@ def _axis_synthesis(lo_band: torch.Tensor, hi_band: torch.Tensor, axis: int, out
     return _rows_back(y, lo_band.shape, axis, out_len)
 
 
+def _axis_pass_graph(lo_band: torch.Tensor, hi_band: torch.Tensor, axis: int, out_len: int, rec_lo_t: torch.Tensor,
+                     rec_hi_t: torch.Tensor) -> torch.Tensor:
+    """One synthesis pass along one axis through :class:`LevelSynthesis` (recorded by autograd), cropped to
+    `out_len` samples; with ``rec := flipped dec`` it is the adjoint of the zero-extension analysis pass."""
+    rl, rh = _axis_rows(lo_band, axis), _axis_rows(hi_band, axis)
+    y = LevelSynthesis.apply(rec_lo_t, rec_hi_t, 1, rl, rh)[:, :out_len]
+    return _rows_back(y, lo_band.shape, axis, out_len)
+
+
 def _tap_corr(c_lo: torch.Tensor, c_hi: torch.Tensor, sig: torch.Tensor, axis: int, filt_len: int) -> torch.Tensor:
     """out[k, t] = sum c_k[.., i, ..] * sig[.., 2 i + t + 2 - L, ..] along `axis` (float64, on the device)."""
+    rl, rh, rs = _axis_rows(c_lo, axis), _axis_rows(c_hi, axis), _axis_rows(sig, axis)
+    return _tap_corr_rows(rl, rh, rs, filt_len)
+
+
+def _tap_corr_rows(rl: torch.Tensor, rh: torch.Tensor, rs: torch.Tensor, filt_len: int) -> torch.Tensor:
+    """:func:`_tap_corr` of contiguous rows ``[R, m]`` (coefficients) and ``[R, n]`` (signal): one wt_tap_corr launch."""
     from . import _native as N
     from .fwt import _dtype_code
 
-    rl, rh, rs = _axis_rows(c_lo, axis), _axis_rows(c_hi, axis), _axis_rows(sig, axis)
-    out = torch.empty(2 * filt_len, dtype=torch.float64, device=sig.device)
-    with torch.cuda.device(sig.device):
-        rc = N.load().wt_tap_corr(_dtype_code(sig.dtype), filt_len, rl.data_ptr(), rh.data_ptr(), rl.stride(0),
+    out = torch.empty(2 * filt_len, dtype=torch.float64, device=rs.device)
+    with torch.cuda.device(rs.device):
+        rc = N.load().wt_tap_corr(_dtype_code(rs.dtype), filt_len, rl.data_ptr(), rh.data_ptr(), rl.stride(0),
                                   rs.data_ptr(), rs.stride(0), rl.shape[0], rl.shape[1], rs.shape[1], out.data_ptr(),
-                                  torch.cuda.current_stream(sig.device).cuda_stream)
+                                  torch.cuda.current_stream(rs.device).cuda_stream)
     N.check(rc, "wt_tap_corr")
     return out.view(2, filt_len)
 
@@ -175,9 +197,13 @@ def _band_index(bits: Sequence[int]) -> int:
 def _tap_grads(bands: Sequence[torch.Tensor], sig: torch.Tensor, ndim: int, lo, hi, synthesis: bool) -> torch.Tensor:
     """Sum over the axes of the tap correlations.  `bands` are the 2^ndim band tensors (gradients for analysis,
     coefficients for synthesis) in the order k = sum_a hi(a) << (ndim-1-a); `sig` is the level input (analysis) or
-    the gradient of the cropped level output (synthesis).  Returns [2, L] float64: row 0 lo taps, row 1 hi taps."""
+    the gradient of the cropped level output (synthesis).  Returns [2, L] float64: row 0 lo taps, row 1 hi taps.
+
+    Given the taps as tensors (grad mode), every pass and correlation is recorded by autograd."""
     import itertools
 
+    if isinstance(lo, torch.Tensor):
+        return _tap_grads_graph(bands, sig, ndim, lo, hi, synthesis)
     L = len(lo)
     total = torch.zeros(2, L, dtype=torch.float64, device=sig.device)
     for a in range(ndim):
@@ -201,6 +227,64 @@ def _tap_grads(bands: Sequence[torch.Tensor], sig: torch.Tensor, ndim: int, lo, 
     return total
 
 
+def _tap_grads_graph(bands, sig: torch.Tensor, ndim: int, lo_t: torch.Tensor, hi_t: torch.Tensor,
+                     synthesis: bool) -> torch.Tensor:
+    """:func:`_tap_grads` with the passes through :class:`LevelSynthesis` and the correlations through
+    :class:`TapCorrelation`, so that the result is differentiable in the bands, the signal and the taps."""
+    import itertools
+
+    rec_lo, rec_hi = (lo_t, hi_t) if synthesis else (_flipped(lo_t), _flipped(hi_t))
+    L = lo_t.numel()
+    terms = []
+    for a in range(ndim):
+        cur = {bits: bands[_band_index(bits)] for bits in itertools.product((0, 1), repeat=ndim)}
+        for a2 in range(ndim):
+            if a2 == a:
+                continue
+            nxt = {}
+            for bits, t in cur.items():
+                if bits[a2] != 0:
+                    continue
+                other = cur[bits[:a2] + (1,) + bits[a2 + 1:]]
+                nxt[bits[:a2] + (None,) + bits[a2 + 1:]] = _axis_pass_graph(t, other, a2, sig.shape[1 + a2], rec_lo,
+                                                                            rec_hi)
+            cur = nxt
+        q_lo = next(t for bits, t in cur.items() if bits[a] == 0)
+        q_hi = next(t for bits, t in cur.items() if bits[a] == 1)
+        terms.append(TapCorrelation.apply(_axis_rows(q_lo, a), _axis_rows(q_hi, a), _axis_rows(sig, a), L))
+    return sum(terms[1:], terms[0])
+
+
+def _flipped(taps: torch.Tensor) -> torch.Tensor:
+    return taps.reshape(-1).flip(0)
+
+
+class TapCorrelation(torch.autograd.Function):
+    """``out[k, t] = sum_{r, i} c_k[r, i] * s[r, 2 i + t + 2 - L]`` of coefficient rows ``c_lo, c_hi [R, m]`` and
+    signal rows ``s [R, n]`` (wt_tap_corr) -> ``[2, L]`` float64.  It is bilinear; for the cotangent ``v [2, L]``
+    ``d s[j] = sum_k sum_i c_k[i] v[k, j - 2 i + L - 2]`` is one synthesis pass of the coefficients with ``rec := v``
+    (its crop of L - 2 samples gives exactly this index), and ``d c_k[i] = sum_t v[k, t] s[2 i + t + 2 - L]`` one
+    zero-extension analysis pass of the signal with ``dec := flipped v``."""
+
+    @staticmethod
+    def forward(ctx, c_lo, c_hi, s, filt_len: int):
+        c_lo, c_hi, s = c_lo.contiguous(), c_hi.contiguous(), s.contiguous()
+        ctx.save_for_backward(c_lo, c_hi, s)
+        return _tap_corr_rows(c_lo, c_hi, s, filt_len)
+
+    @staticmethod
+    def backward(ctx, v):
+        c_lo, c_hi, s = ctx.saved_tensors
+        g_lo = g_hi = g_s = None
+        if ctx.needs_input_grad[2]:
+            g_s = LevelSynthesis.apply(v[0], v[1], 1, c_lo, c_hi)[:, :s.shape[1]]
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            g_lo, g_hi = ZeroLevelAnalysis.apply(s, v[0].flip(0), v[1].flip(0), 1)
+            if g_lo.shape != c_lo.shape:
+                raise AssertionError("TapCorrelation: unexpected coefficient extents")
+        return g_lo, g_hi, g_s, None
+
+
 class ZeroLevelAnalysis(torch.autograd.Function):
     """One analysis level with zero extension: ``x [B, d..] -> 2^ndim bands``; the filters are tensor inputs."""
 
@@ -216,26 +300,37 @@ class ZeroLevelAnalysis(torch.autograd.Function):
         ctx.in_shape = tuple(x.shape)
         ctx.tap_meta = (dec_lo_t.dtype, dec_lo_t.device, tuple(dec_lo_t.shape), dec_hi_t.dtype, dec_hi_t.device,
                         tuple(dec_hi_t.shape))
-        ctx.save_for_backward(x if (dec_lo_t.requires_grad or dec_hi_t.requires_grad) else None)
+        ctx.save_for_backward(x if (dec_lo_t.requires_grad or dec_hi_t.requires_grad) else None, dec_lo_t, dec_hi_t)
         return (approx,) + tuple(details[0])
 
     @staticmethod
     def backward(ctx, *grads):
         ref = next(g for g in grads if g is not None)
         bands = [g.contiguous() if g is not None else torch.zeros_like(ref) for g in grads]
-        x = ctx.saved_tensors[0] if (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]) else None
+        graph = torch.is_grad_enabled()   # create_graph=True: the tap tensors go through the other Functions
+        x = tap_tensors = None
+        if graph or ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            x, *taps = ctx.saved_tensors
+            tap_tensors = tuple(taps) if graph else None
         gx, g_lo, g_hi = _zero_analysis_backward(bands, ctx.in_shape, ctx.taps, ctx.ndim, ctx.tap_meta, x,
-                                                 ctx.needs_input_grad[:3])
+                                                 ctx.needs_input_grad[:3], tap_tensors)
         return gx, g_lo, g_hi, None
 
 
-def _zero_analysis_backward(bands, in_shape, taps, ndim: int, tap_meta, x, needs):
-    """Backward of one zero-extension analysis level of a signal of shape ``in_shape``: (gx, g_dec_lo, g_dec_hi)."""
+def _zero_analysis_backward(bands, in_shape, taps, ndim: int, tap_meta, x, needs, tap_tensors=None):
+    """Backward of one zero-extension analysis level of a signal of shape ``in_shape``: (gx, g_dec_lo, g_dec_hi).
+
+    ``tap_tensors`` (grad mode only): the filters as tensors; the result is then recorded by autograd."""
     from . import fwt
 
     dec_lo, dec_hi = taps
+    if tap_tensors is not None:
+        dec_lo, dec_hi = tap_tensors
     gx = None
-    if needs[0]:
+    if needs[0] and tap_tensors is not None:
+        gx = LevelSynthesis.apply(_flipped(dec_lo), _flipped(dec_hi), ndim, *bands)
+        gx = gx[(slice(None),) + tuple(slice(0, n) for n in in_shape[1:])]
+    elif needs[0]:
         # adjoint of (zero pad -> stride-2 correlation) = transposed convolution with the same kernel,
         # cropped by the pad: the synthesis kernel with rec := flipped dec
         wav = (None, None, list(dec_lo)[::-1], list(dec_hi)[::-1])
@@ -271,7 +366,7 @@ class ModeLevelAnalysis(torch.autograd.Function):
         ctx.in_shape = tuple(x.shape)
         ctx.tap_meta = (dec_lo_t.dtype, dec_lo_t.device, tuple(dec_lo_t.shape), dec_hi_t.dtype, dec_hi_t.device,
                         tuple(dec_hi_t.shape))
-        ctx.save_for_backward(x if (dec_lo_t.requires_grad or dec_hi_t.requires_grad) else None)
+        ctx.save_for_backward(x if (dec_lo_t.requires_grad or dec_hi_t.requires_grad) else None, dec_lo_t, dec_hi_t)
         return (approx,) + tuple(details[0])
 
     @staticmethod
@@ -295,8 +390,9 @@ class ModeLevelAnalysis(torch.autograd.Function):
         xp = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             xp = extend(ctx.saved_tensors[0], ndim, L, mode)   # recomputed here instead of kept from the forward pass
+        tap_tensors = tuple(ctx.saved_tensors[1:]) if torch.is_grad_enabled() else None   # create_graph=True
         gxp, g_lo, g_hi = _zero_analysis_backward(bands, (ctx.in_shape[0],) + ext_dims, ctx.taps, ndim, ctx.tap_meta, xp,
-                                                  ctx.needs_input_grad[:3])
+                                                  ctx.needs_input_grad[:3], tap_tensors)
         gx = fold_extension(gxp, dims, L, mode) if gxp is not None else None
         return gx, g_lo, g_hi, None, None
 
@@ -318,26 +414,32 @@ class LevelSynthesis(torch.autograd.Function):
         ctx.tap_meta = (rec_lo_t.dtype, rec_lo_t.device, tuple(rec_lo_t.shape), rec_hi_t.dtype, rec_hi_t.device,
                         tuple(rec_hi_t.shape))
         if rec_lo_t.requires_grad or rec_hi_t.requires_grad:
-            ctx.save_for_backward(*bands)
+            ctx.save_for_backward(rec_lo_t, rec_hi_t, *bands)
+        else:
+            ctx.save_for_backward(rec_lo_t, rec_hi_t)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         from . import fwt
 
-        rec_lo, rec_hi = ctx.taps
+        graph = torch.is_grad_enabled()   # create_graph=True: the tap tensors go through the other Functions
+        rec_lo, rec_hi = ctx.saved_tensors[:2] if graph else ctx.taps
         gy = gy.contiguous()
         out_bands = (None,) * (2 ** ctx.ndim)
         if any(ctx.needs_input_grad[3:]):
             # adjoint of (transposed convolution -> crop) = zero-extension analysis with dec := flipped rec
-            wav = (list(rec_lo)[::-1], list(rec_hi)[::-1], None, None)
-            approx, details, _ = fwt._analysis(gy, wav, "zero", 1, None, ctx.ndim)
-            out = [approx] + list(details[0])
+            if graph:
+                out = ZeroLevelAnalysis.apply(gy, _flipped(rec_lo), _flipped(rec_hi), ctx.ndim)
+            else:
+                wav = (list(rec_lo)[::-1], list(rec_hi)[::-1], None, None)
+                approx, details, _ = fwt._analysis(gy, wav, "zero", 1, None, ctx.ndim)
+                out = [approx] + list(details[0])
             sl = (slice(None),) + tuple(slice(0, n) for n in ctx.coeff_shape[1:])
             out_bands = tuple(t[sl] for t in out)
         g_lo = g_hi = None
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
-            bands = [b.contiguous() for b in ctx.saved_tensors]
+            bands = [b.contiguous() for b in ctx.saved_tensors[2:]]
             d = _tap_grads(bands, gy, ctx.ndim, rec_lo, rec_hi, synthesis=True)       # d rec[t] = out[t]
             ldt, ldev, lshape, hdt, hdev, hshape = ctx.tap_meta
             if ctx.needs_input_grad[0]:

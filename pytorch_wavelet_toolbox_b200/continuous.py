@@ -321,7 +321,23 @@ class _CwtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
+        if torch.is_grad_enabled():   # create_graph=True: the adjoint as a differentiable map
+            return _CwtAdjointFunction.apply(gy, ctx.plan, ctx.dtype), None
         return run_adjoint(gy, ctx.plan, ctx.dtype), None
+
+
+class _CwtAdjointFunction(torch.autograd.Function):
+    """``gy -> Re(A^H gy)`` in the data's dtype.  Under torch's convention for complex gradients the adjoint of this
+    real-linear map is ``u -> A u``: the forward transform again, in float64 or complex128 like ``gy``."""
+
+    @staticmethod
+    def forward(ctx, gy, plan, dtype):
+        ctx.plan = plan
+        return run_adjoint(gy, plan, dtype)
+
+    @staticmethod
+    def backward(ctx, u):
+        return _CwtFunction.apply(u, ctx.plan), None, None
 
 
 # --------------------------------------------------------------------------------------

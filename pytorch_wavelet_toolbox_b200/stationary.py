@@ -22,6 +22,7 @@ from typing import Any, Optional, Sequence
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from . import _native as N
 from ._shape import AxisHint, check_dtype, check_tensor, fold, round_up, unfold
@@ -186,8 +187,26 @@ def run_synthesis(approx: torch.Tensor, details: Sequence[torch.Tensor], g_lo, g
 
 
 # --------------------------------------------------------------------------------------
-# autograd: each direction's backward is the other kernel with the adjoint taps and the transposed tables
+# autograd: each direction's backward is the other kernel with the adjoint taps and the transposed tables.  In grad
+# mode (create_graph=True) that backward runs as a Function of its own whose backward is the forward kernel again, so
+# gradients of any order reach the data.
 # --------------------------------------------------------------------------------------
+def _swt_adjoint(g: torch.Tensor, fb, levels: int, L: int, n: int) -> torch.Tensor:
+    """Adjoint of swt: packed ``[B, levels + 1, pitch]`` gradient -> ``[B, n]`` (the pitch padding is not read)."""
+    g = g.contiguous()
+    f_lo, f_hi = _window_taps(fb, g.dtype, inverse=False)
+    details = [g[:, k, :n] for k in range(1, levels + 1)]
+    return run_synthesis(g[:, 0, :n], details, f_lo, f_hi, L, tables_inverse=False, transpose=True)
+
+
+def _iswt_adjoint(gy: torch.Tensor, fb, levels: int, L: int) -> tuple:
+    """Adjoint of iswt: ``[B, n]`` gradient -> the gradients of approx and the ``levels`` details."""
+    f_lo, f_hi = _window_taps(fb, gy.dtype, inverse=True)
+    n = gy.shape[-1]
+    packed = run_analysis(gy.contiguous(), f_lo, f_hi, levels, L, tables_inverse=True, transpose=True)
+    return tuple(packed[:, k, :n] for k in range(levels + 1))
+
+
 class _SwtFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, fb, levels, L):
@@ -197,11 +216,24 @@ class _SwtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        g, n = g.contiguous(), ctx.n
-        f_lo, f_hi = _window_taps(ctx.fb, g.dtype, inverse=False)
-        details = [g[:, k, :n] for k in range(1, ctx.levels + 1)]
-        gx = run_synthesis(g[:, 0, :n], details, f_lo, f_hi, ctx.L, tables_inverse=False, transpose=True)
-        return gx, None, None, None
+        if torch.is_grad_enabled():
+            return _SwtAdjointFunction.apply(g, ctx.fb, ctx.levels, ctx.L, ctx.n), None, None, None
+        return _swt_adjoint(g, ctx.fb, ctx.levels, ctx.L, ctx.n), None, None, None
+
+
+class _SwtAdjointFunction(torch.autograd.Function):
+    """The backward pass of swt as a differentiable map; its own adjoint is swt, written into the packed layout
+    with zeros in the pitch padding (those entries never reach the data gradient)."""
+
+    @staticmethod
+    def forward(ctx, g, fb, levels, L, n):
+        ctx.fb, ctx.levels, ctx.L, ctx.n, ctx.pitch = fb, levels, L, n, g.shape[-1]
+        return _swt_adjoint(g, fb, levels, L, n)
+
+    @staticmethod
+    def backward(ctx, u):
+        packed = _SwtFunction.apply(u, ctx.fb, ctx.levels, ctx.L)
+        return F.pad(packed[..., :ctx.n], (0, ctx.pitch - ctx.n)), None, None, None, None
 
 
 class _IswtFunction(torch.autograd.Function):
@@ -213,10 +245,22 @@ class _IswtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        f_lo, f_hi = _window_taps(ctx.fb, gy.dtype, inverse=True)
-        n = gy.shape[-1]
-        packed = run_analysis(gy.contiguous(), f_lo, f_hi, ctx.levels, ctx.L, tables_inverse=True, transpose=True)
-        return (None, None) + tuple(packed[:, k, :n] for k in range(ctx.levels + 1))
+        if torch.is_grad_enabled():
+            return (None, None) + _IswtAdjointFunction.apply(gy, ctx.fb, ctx.levels, ctx.L)
+        return (None, None) + _iswt_adjoint(gy, ctx.fb, ctx.levels, ctx.L)
+
+
+class _IswtAdjointFunction(torch.autograd.Function):
+    """The backward pass of iswt as a differentiable map; its own adjoint is iswt."""
+
+    @staticmethod
+    def forward(ctx, gy, fb, levels, L):
+        ctx.fb, ctx.L = fb, L
+        return _iswt_adjoint(gy, fb, levels, L)
+
+    @staticmethod
+    def backward(ctx, *us):
+        return _IswtFunction.apply(ctx.fb, ctx.L, *[u.contiguous() for u in us]), None, None, None
 
 
 def _check_taps_without_grad(wav: Any) -> None:
