@@ -321,9 +321,7 @@ class _CwtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        if torch.is_grad_enabled():   # create_graph=True: the adjoint as a differentiable map
-            return _CwtAdjointFunction.apply(gy, ctx.plan, ctx.dtype), None
-        return run_adjoint(gy, ctx.plan, ctx.dtype), None
+        return _CwtAdjointFunction.apply(gy, ctx.plan, ctx.dtype), None
 
 
 class _CwtAdjointFunction(torch.autograd.Function):

@@ -187,9 +187,9 @@ def run_synthesis(approx: torch.Tensor, details: Sequence[torch.Tensor], g_lo, g
 
 
 # --------------------------------------------------------------------------------------
-# autograd: each direction's backward is the other kernel with the adjoint taps and the transposed tables.  In grad
-# mode (create_graph=True) that backward runs as a Function of its own whose backward is the forward kernel again, so
-# gradients of any order reach the data.
+# autograd: each direction's backward is the other kernel with the adjoint taps and the transposed tables, run as a
+# Function of its own whose backward is the forward kernel again, so in grad mode (create_graph=True) gradients of any
+# order reach the data.
 # --------------------------------------------------------------------------------------
 def _swt_adjoint(g: torch.Tensor, fb, levels: int, L: int, n: int) -> torch.Tensor:
     """Adjoint of swt: packed ``[B, levels + 1, pitch]`` gradient -> ``[B, n]`` (the pitch padding is not read)."""
@@ -216,9 +216,7 @@ class _SwtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        if torch.is_grad_enabled():
-            return _SwtAdjointFunction.apply(g, ctx.fb, ctx.levels, ctx.L, ctx.n), None, None, None
-        return _swt_adjoint(g, ctx.fb, ctx.levels, ctx.L, ctx.n), None, None, None
+        return _SwtAdjointFunction.apply(g, ctx.fb, ctx.levels, ctx.L, ctx.n), None, None, None
 
 
 class _SwtAdjointFunction(torch.autograd.Function):
@@ -245,9 +243,7 @@ class _IswtFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        if torch.is_grad_enabled():
-            return (None, None) + _IswtAdjointFunction.apply(gy, ctx.fb, ctx.levels, ctx.L)
-        return (None, None) + _iswt_adjoint(gy, ctx.fb, ctx.levels, ctx.L)
+        return (None, None) + _IswtAdjointFunction.apply(gy, ctx.fb, ctx.levels, ctx.L)
 
 
 class _IswtAdjointFunction(torch.autograd.Function):

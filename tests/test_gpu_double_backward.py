@@ -11,6 +11,8 @@ differentiated again, as the reference's chain of torch operators can.  This fil
   gradients of the weights (and of the filters, where they are learnable) match the float64 oracle ports
   (oracle/ptwt_port.py, swt_port.py, cwt_port.py), which are torch operators and can be differentiated twice;
 * a Hessian-vector product of a reconstruction loss with respect to learnable filters matches the oracle's;
+* first-order gradients taken with ``create_graph=False`` (taps as floats, no graph) and ``create_graph=True`` (taps as
+  tensors, recorded) agree: one backward path serves both;
 * the profiler shows what the second-order pass runs: the library's analysis, synthesis, tap-correlation, swt and cwt
   kernels, and otherwise only PyTorch's elementwise, copy, fill, pad and index kernels; never cuDNN, cuFFT, cuBLAS or
   CUTLASS.
@@ -110,6 +112,42 @@ def test_gradgradcheck_cwt(wavelet):
     x = _rand((2, 45), seed=6, device=DEV).requires_grad_(True)
     scales = np.arange(1, 7)
     assert gradgradcheck(lambda x: wt.cwt(x, scales, wavelet)[0], (x,), fast_mode=True)
+
+
+# ---- the same first-order gradients with and without a graph ---------------------------------------------------------
+#: odd and even extents, two levels of db3 in every mode
+_AGREE = {1: (3, 67), 2: (2, 33, 40), 3: (1, 17, 20, 15)}
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, F64], ids=["f32", "f64"])
+@pytest.mark.parametrize("learnable", [False, True], ids=["data", "learnable"])
+@pytest.mark.parametrize("ndim", [1, 2, 3])
+def test_gradients_agree_with_and_without_create_graph(ndim, learnable, dtype):
+    """A backward pass without grad mode runs on the filters as floats, one in grad mode on the filters as tensors;
+    both give the same gradients: the data gradient bit for bit, the filter gradients to the round-off of the tap
+    correlation's float64 atomics."""
+    dec, rec, _, _ = _TRANSFORMS[ndim]
+    x0 = _rand(_AGREE[ndim], dtype, seed=30 + ndim, device=DEV)
+    tol = 1e-12 if dtype == F64 else TOL[dtype]
+    for mode in MODES:
+        results = []
+        for create_graph in (False, True):
+            x = x0.clone().requires_grad_(True)
+            taps = _taps("db3", DEV, dtype) if learnable else []
+            w = wt.WaveletTensorTuple(*taps) if learnable else "db3"
+            c = dec(x, w, mode=mode, level=2)
+            outs = flatten_coeffs(c) + [rec(c, w)]
+            # weights that require grad: under create_graph=True every gradient then carries a graph
+            weights = [_rand(t.shape, dtype, seed=40 + j, device=DEV).requires_grad_(True) for j, t in enumerate(outs)]
+            loss = sum((t * u).sum() for t, u in zip(outs, weights))
+            grads = torch.autograd.grad(loss, [x] + taps, create_graph=create_graph)
+            assert all(g.requires_grad == create_graph for g in grads), f"{mode}: create_graph={create_graph}"
+            results.append([g.detach() for g in grads])
+        (gx1, *gt1), (gx2, *gt2) = results
+        assert torch.equal(gx1, gx2), f"{ndim}-D {mode}: data gradients differ"
+        for k, (a, b) in enumerate(zip(gt1, gt2)):
+            err, scale = float((a - b).abs().max()), float(a.abs().max())
+            assert err <= tol * scale, f"{ndim}-D {mode}: filter {k} gradients differ by {err:.3e} > {tol:.0e} * {scale:.3e}"
 
 
 # ---- R1 penalty at user sizes ----------------------------------------------------------------------------------------

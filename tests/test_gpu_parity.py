@@ -459,7 +459,7 @@ def test_filter_tap_gradients_match_the_reference_operators(mode):
 @pytest.mark.parametrize("mode", ["constant", "symmetric", "periodic", "reflect"])
 def test_autograd_extension_longer_than_the_signal(mode):
     """Under grad the boundary extension runs inside the analysis kernel and the backward pass folds the gradient of
-    the extended signal (ModeLevelAnalysis): short signals whose extension wraps more than once, odd lengths, all the
+    the extended signal (LevelAnalysis outside zero mode): short signals whose extension wraps more than once, odd lengths, all the
     levels the signal allows -- data and filter gradients against the oracle's torch-operator chain."""
     g = torch.Generator().manual_seed(47)
     for n, wav, level in ((9, "db4", 1), (11, "db3", 2), (6, "db2", 1), (23, "db5", 1)):
