@@ -18,6 +18,9 @@ ROOT = HERE.parent.parent
 LIB = HERE / "libwtb200.so"
 SOURCES = [HERE / "wtb200.cu"]
 HEADERS = sorted(HERE.glob("*.cuh")) + [ROOT / "include" / "wtb200.h"]
+# traffic twin of fwd2d_wpair_kernel for tools/time_wpair_ceiling.py: a separate object, never part of the library
+TWIN = ROOT / "tools" / "wpair_twin" / "libwpair_twin.so"
+TWIN_SOURCES = [ROOT / "tools" / "wpair_twin" / "wpair_twin.cu"]
 
 
 def _nvcc() -> str:
@@ -27,16 +30,22 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found: cannot build libwtb200.so")
 
 
-def needs_build() -> bool:
-    if not LIB.exists():
+def needs_build(out: Path = LIB, sources: list[Path] = SOURCES) -> bool:
+    if not out.exists():
         return True
-    t = LIB.stat().st_mtime
-    return any(p.stat().st_mtime > t for p in SOURCES + HEADERS + [Path(__file__)])
+    t = out.stat().st_mtime
+    return any(p.stat().st_mtime > t for p in sources + HEADERS + [Path(__file__)])
 
 
 def build(force: bool = False, verbose: bool = False, extra: list[str] | None = None) -> Path:
-    if not force and not needs_build():
-        return LIB
+    """Build libwtb200.so and the wpair traffic twin; returns the library's path."""
+    _build_one(TWIN, TWIN_SOURCES, force, verbose, extra)
+    return _build_one(LIB, SOURCES, force, verbose, extra)
+
+
+def _build_one(out: Path, sources: list[Path], force: bool, verbose: bool, extra: list[str] | None) -> Path:
+    if not force and not needs_build(out, sources):
+        return out
     cmd = [
         _nvcc(), "-O3", "-std=c++17",
         "-gencode", "arch=compute_90a,code=sm_90a",
@@ -44,8 +53,8 @@ def build(force: bool = False, verbose: bool = False, extra: list[str] | None = 
         "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
         "--expt-relaxed-constexpr",
         "-shared", "-cudart", "static",
-        "-o", str(LIB),
-    ] + [str(s) for s in SOURCES]
+        "-o", str(out),
+    ] + [str(s) for s in sources]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     if extra:
@@ -55,7 +64,7 @@ def build(force: bool = False, verbose: bool = False, extra: list[str] | None = 
         raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + proc.stdout + proc.stderr)
     if verbose:
         sys.stderr.write(proc.stdout + proc.stderr)
-    return LIB
+    return out
 
 
 if __name__ == "__main__":

@@ -6,7 +6,8 @@
 // level's approximation band to HBM: with one launch per level that band makes a round trip
 // (+25 % traffic at the first level, 1.33x over the whole pyramid).
 //
-// Structure (no CTA-wide barrier anywhere; a CTA is ONE warp):
+// Structure (no CTA-wide barrier anywhere; a CTA is ONE warp; adjacent strips form a cluster that passes a split
+// cluster barrier once per group, so that they stream their rows in step):
 //   * a warp owns a strip of 128 level-1 columns (lane <-> 4 adjacent columns) and a segment of rows
 //     and marches down it; input rows arrive by TMA (cp.async.bulk.tensor, 8-byte elements so that
 //     the 264-sample rows fit one box) in groups of 4 rows into a private 3-stage ring, completion on
@@ -77,6 +78,10 @@ struct WPairGeom {
     static_assert(TILE_W % 4 == 0 && TILE_W / 2 <= 256, "tile row must fit one TMA box of 8-byte elements");
     static_assert(RING >= L, "ring too small for the window of one output row");
 };
+
+// split cluster barrier (a CTA launched without a cluster is a cluster of one)
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
 
 // lo[c], hi[c] for NC consecutive outputs from the register window w (see row_filter)
 template <int L, int NC, int OFF, int NW>
@@ -252,6 +257,10 @@ fwd2d_wpair_kernel(const __grid_constant__ WPairParams p, const __grid_constant_
         for (int u = 0; u < UNR; ++u) {
             const int g = g0 + u;
             if (g >= ngroups) break;
+            // Adjacent strips of one segment form a cluster and march in step, at most one group apart: their
+            // row pieces then reach DRAM together as long contiguous runs.  Left to drift apart, the same
+            // traffic streams at about 2.1 instead of 2.7 TB/s on an H100 (tools/time_wpair_ceiling.py).
+            if (g > 0) cluster_wait();
             float* tile = s_tile + stage * STG_F;
             mbar_wait(&bars[stage], par);
             const int rbase = r_in0 + g * ROWS;
@@ -366,6 +375,7 @@ fwd2d_wpair_kernel(const __grid_constant__ WPairParams p, const __grid_constant_
                 tma_load_3d(tile, &tmap, &bars[stage], c_in0 / 2, r_in0 + (g + NSTG) * ROWS, b);
             }
             if (++stage == NSTG) { stage = 0; par ^= 1u; }
+            cluster_arrive();
 
             // ---- level 2 column pass: every output row whose L ring lines exist ----------------------------
             while (K2 < Y1) {
@@ -405,6 +415,7 @@ fwd2d_wpair_kernel(const __grid_constant__ WPairParams p, const __grid_constant_
             }
         }
     }
+    if (ngroups > 0) cluster_wait();   // pairs the last arrive
 }
 
 // ------------------------------------------------------------------------------------------
@@ -428,13 +439,13 @@ static bool make_tmap_3d_pairs(CUtensorMap* map, const float* base, int64_t B, i
     return r == CUDA_SUCCESS;
 }
 
-// Returns true when the two levels were launched here (*err carries the launch status).
-template <int L, int NSTG, int MINB>
-static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
-                                 const wt_level& l2, int mode, const Taps<float>& taps, cudaStream_t st,
-                                 uint64_t* launches, cudaError_t* err) {
+// Parameters, tensor map and strip count of one levels-1-2 call; false when the kernel does not take these shapes,
+// strides or mode.  The grid is (nstrip, batch, p.nseg).
+template <int L, int NSTG>
+static bool wpair_plan(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
+                       const wt_level& l2, int mode, const Taps<float>& taps, WPairParams& p, CUtensorMap& tmap,
+                       int& nstrip) {
     using Gm = WPairGeom<L, NSTG>;
-    WPairParams p;
     memset(&p, 0, sizeof(p));
     p.x = x; p.x_bs = x_bs; p.x_rs = x_rs; p.H = H; p.W = W;
     p.Mh1 = (int)l1.dims[0]; p.Mw1 = (int)l1.dims[1]; p.Mh2 = (int)l2.dims[0]; p.Mw2 = (int)l2.dims[1];
@@ -455,7 +466,7 @@ static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_
     for (int k = 0; k < 4; ++k)
         if (((uintptr_t)p.o2[k] & 7) || (p.o2_bs[k] & 1) || (p.o2_rs[k] & 1) || p.o2_rs[k] < (p.Mw2 + 1) / 2 * 2) return false;
     // strips: the (possibly shifted) last strip must still reach the last level-2 column
-    const int nstrip = (p.Mw2 + Gm::TW2 - 1) / Gm::TW2;
+    nstrip = (p.Mw2 + Gm::TW2 - 1) / Gm::TW2;
     {
         int X0 = (nstrip - 1) * Gm::TW2;
         const int lim = (p.Mw1 - L + Gm::HL1) / 2;
@@ -472,7 +483,6 @@ static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_
         p.vl[m] = make_float2(taps.lo[m], taps.lo[m]);
         p.vh[m] = make_float2(taps.hi[m], taps.hi[m]);
     }
-    CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     if (!make_tmap_3d_pairs(&tmap, x, B, H, W, x_bs, x_rs, Gm::TILE_W / 2, Gm::ROWS)) return false;
     // segments: long ones (restart overhead ~3 %) first, then geometrically shorter ones that fill the tail of the
@@ -496,16 +506,40 @@ static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_
         if (y < p.Mh2) p.seg_start[n] = p.Mh2;   // table full: the last segment takes the rest
         p.nseg = n;
     }
+    return true;
+}
+
+// Returns true when the two levels were launched here (*err carries the launch status).
+template <int L, int NSTG, int MINB>
+static bool launch_fwd2d_wpair_t(const float* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level& l1,
+                                 const wt_level& l2, int mode, const Taps<float>& taps, cudaStream_t st,
+                                 uint64_t* launches, cudaError_t* err) {
+    using Gm = WPairGeom<L, NSTG>;
+    WPairParams p;
+    CUtensorMap tmap;
+    int nstrip = 0;
+    if (!wpair_plan<L, NSTG>(x, B, H, W, x_bs, x_rs, l1, l2, mode, taps, p, tmap, nstrip)) return false;
     const int nseg = p.nseg;
     auto kern = fwd2d_wpair_kernel<L, NSTG, MINB>;
     const cudaError_t attr_err = ensure_dyn_smem(kern, (size_t)Gm::SMEM);
     if (attr_err != cudaSuccess) { *err = attr_err; return true; }
     *err = cudaSuccess;
+    // clusters of adjacent strips (see the cluster barrier in the kernel): the largest of 6, 3, 2 that divides nstrip
+    const int cl = nstrip % 6 == 0 ? 6 : nstrip % 3 == 0 ? 3 : nstrip % 2 == 0 ? 2 : 1;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cl; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     for (int64_t b0 = 0; b0 < B; b0 += 65535) {
         p.batch0 = (int)b0;
         const int nb = (int)((B - b0) < 65535 ? (B - b0) : 65535);
-        dim3 grid(nstrip, nb, nseg);
-        kern<<<grid, 32, Gm::SMEM, st>>>(p, tmap);
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(nstrip, nb, nseg);
+        cfg.blockDim = dim3(32, 1, 1);
+        cfg.dynamicSmemBytes = Gm::SMEM;
+        cfg.stream = st;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        cudaLaunchKernelEx(&cfg, kern, p, tmap);
         ++*launches;
         *err = cudaGetLastError();
         if (*err != cudaSuccess) return true;
