@@ -215,6 +215,28 @@ fwd2d_wpair_kernel(const __grid_constant__ WPairParams p, const __grid_constant_
     const bool need_patch = (p.mode != WT_MODE_ZERO) || (p.W & 1);
     const bool edge_in = need_patch && (c_in0 < 0 || c_in0 + TILE_W > p.W);   // warp-uniform
     const bool edge_a = cA0 < 0 || cA0 + TW1 > p.Mw1;                         // warp-uniform
+    // Column patch of the edge strips' staged rows (rows in range): the L samples next to each border are all any valid
+    // output reads.  The same for every row and group: lane q < (at most 2L) patches position cp_t of each staged row
+    // from position cp_s of the same row (-1: zero).  The sources are in-range samples, normally staged in the tile
+    // already, so the patch is a shared-memory copy; a global-memory round trip in every group of the edge strips
+    // would hold back their whole cluster (the cluster barrier waits for its slowest strip).  When a source lies outside
+    // the tile, the whole warp reads its sources from global memory instead.
+    int cp_t = -1, cp_s = -1;
+    bool cpatch_staged = true;
+    if (edge_in) {
+        const int nl = c_in0 < 0 ? -c_in0 : 0;
+        const int l0 = max(nl - L, 0);
+        const int r0 = min(max(p.W - c_in0, 0), TILE_W), r1 = min(r0 + L, TILE_W);
+        const int wl = nl - l0, wb = wl + (r1 - r0);
+        bool staged = true;
+        if (lane < wb) {   // wb <= 2L <= 32
+            cp_t = lane < wl ? l0 + lane : r0 + (lane - wl);
+            const int sc = ext_index32(c_in0 + cp_t, p.W, p.mode);
+            cp_s = sc < 0 ? -1 : sc - c_in0;   // an in-range column: never a patched position
+            staged = sc < 0 || (cp_s >= 0 && cp_s < TILE_W);
+        }
+        cpatch_staged = __all_sync(0xffffffffu, staged);
+    }
 
     // level-1 stores: this lane's 4 columns, running pointer = row `produced` of band 1
     const int col1 = cA0 + 4 * lane;
@@ -279,16 +301,16 @@ fwd2d_wpair_kernel(const __grid_constant__ WPairParams p, const __grid_constant_
                     }
                     __syncwarp();
                 } else if (edge_in) {
-                    // columns only: the L samples next to each border are all any valid output reads
-                    const int nl = c_in0 < 0 ? -c_in0 : 0;
-                    const int l0 = max(nl - L, 0);
-                    const int r0 = min(max(p.W - c_in0, 0), TILE_W), r1 = min(r0 + L, TILE_W);
-                    const int wl = nl - l0, wb = wl + (r1 - r0);
-                    for (int idx = lane; idx < ROWS * wb; idx += 32) {
-                        const int rr = idx / wb, q = idx - rr * wb;
-                        const int t = q < wl ? l0 + q : r0 + (q - wl);
-                        const int sc = ext_index32(c_in0 + t, p.W, p.mode);
-                        tile[rr * TILE_W + t] = sc >= 0 ? __ldg(xb + (int64_t)(rbase + rr) * p.x_rs + sc) : 0.f;
+                    if (cpatch_staged) {
+                        if (cp_t >= 0) {
+#pragma unroll
+                            for (int rr = 0; rr < ROWS; ++rr)
+                                tile[rr * TILE_W + cp_t] = cp_s >= 0 ? tile[rr * TILE_W + cp_s] : 0.f;
+                        }
+                    } else if (cp_t >= 0) {
+                        const int sc = ext_index32(c_in0 + cp_t, p.W, p.mode);
+                        for (int rr = 0; rr < ROWS; ++rr)
+                            tile[rr * TILE_W + cp_t] = sc >= 0 ? __ldg(xb + (int64_t)(rbase + rr) * p.x_rs + sc) : 0.f;
                     }
                     __syncwarp();
                 }

@@ -6,6 +6,9 @@
 // filtering: every stored value is a plain sum of staged samples.  Its rate is the best this access pattern reaches
 // at the given occupancy, which tells the cost of the real kernel's arithmetic and latency apart from that of its
 // traffic (tools/time_wpair_ceiling.py).  Boundary patching is left out: it touches a few edge strips only.
+// It can keep its strips in step the way the kernel does (one-warp CTAs in a cluster, split cluster barrier) or as
+// warps of one CTA (named barrier), and wpair_kernel_fwd launches the real kernel at the same cluster size and
+// CTAs per SM, so the three can be timed side by side.
 //
 // Built as its own shared object (pytorch_wavelet_toolbox_b200/csrc/build.py), never into libwtb200.so.
 #include <atomic>
@@ -49,7 +52,9 @@ __device__ __forceinline__ void twin_load(void* dst, const CUtensorMap* map, uin
 
 // WPC > 1: a CTA of WPC warps runs WPC adjacent strips (each warp with its own ring, as one CTA of the real kernel)
 // and a named barrier after every group keeps them in lockstep.
-template <int L, int NSTG, int HINT, int WPC = 1>
+// CSYNC (one-warp CTAs launched as clusters): 1 = the kernel's split cluster barrier (arrive after the refill, wait
+// before the next group); 2 = the same barrier not split (wait right after the arrive).
+template <int L, int NSTG, int HINT, int WPC = 1, int CSYNC = 0>
 __global__ void __launch_bounds__(32 * WPC) wpair_twin_kernel(const __grid_constant__ WPairParams p,
                                                               const __grid_constant__ CUtensorMap tmap) {
     using Gm = WPairGeom<L, NSTG>;
@@ -121,6 +126,7 @@ __global__ void __launch_bounds__(32 * WPC) wpair_twin_kernel(const __grid_const
     float* const ring_lane = s_ring + 2 * lane;
 
     for (int g = 0; g < ngroups; ++g) {
+        if (CSYNC == 1 && g > 0) cluster_wait();
         float* tile = s_tile + stage * STG_F;
         mbar_wait(&bars[stage], par);
         const int a0 = a_start + 2 * g - (NA - 1);
@@ -173,6 +179,8 @@ __global__ void __launch_bounds__(32 * WPC) wpair_twin_kernel(const __grid_const
         }
         if (++stage == NSTG) { stage = 0; par ^= 1u; }
         if (WPC > 1) asm volatile("bar.sync 1, %0;" ::"r"(32 * WPC) : "memory");
+        if (CSYNC) cluster_arrive();
+        if (CSYNC == 2) cluster_wait();
 
         while (K2 < Y1) {
             const int vb = 2 * K2 - HALO;
@@ -195,15 +203,61 @@ __global__ void __launch_bounds__(32 * WPC) wpair_twin_kernel(const __grid_const
             ++K2;
         }
     }
+    if (CSYNC == 1 && ngroups > 0) cluster_wait();   // pairs the last arrive
+}
+
+// Dynamic shared memory of `w` warps' worth of `smem` bytes each, padded so that at most ctas_per_sm warps fit on an
+// SM when ctas_per_sm > 0 (228 KB of shared memory per SM, 1 KB of it reserved per CTA).
+static size_t twin_smem(size_t smem, int ctas_per_sm, int w) {
+    smem = (smem + 127) / 128 * 128 * w;
+    if (ctas_per_sm > 0) {
+        const size_t pad = (size_t)(228 * 1024 / (ctas_per_sm / w) - 1024);
+        if (pad > smem) smem = pad;
+    }
+    return smem;
+}
+
+// Launches kern over (ceil(nstrip / w), batch, nseg) CTAs of w warps, as clusters of `cluster` CTAs along x.
+template <typename K>
+static int twin_launch(K kern, const WPairParams& p0, const CUtensorMap& tmap, int nstrip, int64_t B, size_t smem,
+                       int w, int cluster, cudaStream_t st) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess && cluster > 8) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    if (e != cudaSuccess) return (int)e;
+    const int gx = (nstrip + w - 1) / w;
+    if (gx % cluster) return -1;
+    WPairParams p = p0;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    for (int64_t b0 = 0; b0 < B; b0 += 65535) {
+        p.batch0 = (int)b0;
+        const int nb = (int)((B - b0) < 65535 ? (B - b0) : 65535);
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(gx, nb, p.nseg);
+        cfg.blockDim = dim3(32 * w, 1, 1);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        cudaLaunchKernelEx(&cfg, kern, p, tmap);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+    }
+    return 0;
 }
 
 }  // namespace wtb
 
 // Launches the twin of fwd2d_wpair_kernel<8, nstg, *> for levels 1-2 described by lv[0], lv[1] (the wt_level layout
 // of wt_dwt_fwd).  ctas_per_sm > 0 pads the dynamic shared memory so that at most that many CTAs fit on an SM.
-// hint and wpc select HINT and WPC of wpair_twin_kernel (ctas_per_sm then counts warps).  Returns 0, -1 when the real kernel would decline these shapes, or the CUDA error code.
-extern "C" int wpair_twin_fwd(int nstg, int ctas_per_sm, int hint, int wpc, const float* x, int64_t B, int H, int W, int64_t x_bs,
-                              int64_t x_rs, const wt_level* lv, int mode, void* stream) {
+// hint and wpc select HINT and WPC of wpair_twin_kernel (ctas_per_sm then counts warps).  cluster > 1 launches
+// one-warp CTAs as clusters of that many adjacent strips, kept in step by the kernel's split cluster barrier
+// (csync = 1) or by the same barrier not split (csync = 2).  Returns 0, -1 when the real kernel would decline these
+// shapes or the strip count is not a multiple of the cluster size, or the CUDA error code.
+extern "C" int wpair_twin_fwd(int nstg, int ctas_per_sm, int hint, int wpc, int cluster, int csync, const float* x,
+                              int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, const wt_level* lv, int mode,
+                              void* stream) {
     using namespace wtb;
     WPairParams p;
     CUtensorMap tmap;
@@ -213,21 +267,7 @@ extern "C" int wpair_twin_fwd(int nstg, int ctas_per_sm, int hint, int wpc, cons
     const cudaStream_t st = (cudaStream_t)stream;
     auto run = [&](auto kern, size_t smem, bool ok, int w) -> int {
         if (!ok) return -1;
-        smem = (smem + 127) / 128 * 128 * w;
-        if (ctas_per_sm > 0) {   // 228 KB of shared memory per SM, 1 KB of it reserved per CTA
-            const size_t pad = (size_t)(228 * 1024 / (ctas_per_sm / w) - 1024);
-            if (pad > smem) smem = pad;
-        }
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return (int)e;
-        for (int64_t b0 = 0; b0 < B; b0 += 65535) {
-            p.batch0 = (int)b0;
-            const int nb = (int)((B - b0) < 65535 ? (B - b0) : 65535);
-            kern<<<dim3((nstrip + w - 1) / w, nb, p.nseg), 32 * w, smem, st>>>(p, tmap);
-            e = cudaGetLastError();
-            if (e != cudaSuccess) return (int)e;
-        }
-        return 0;
+        return twin_launch(kern, p, tmap, nstrip, B, twin_smem(smem, ctas_per_sm, w), w, w > 1 ? 1 : cluster, st);
     };
     if (nstg == 3)
         return run(wpair_twin_kernel<8, 3, 0>, (size_t)WPairGeom<8, 3>::SMEM,
@@ -237,10 +277,37 @@ extern "C" int wpair_twin_fwd(int nstg, int ctas_per_sm, int hint, int wpc, cons
     if (wpc == 2) return run(wpair_twin_kernel<8, 2, 0, 2>, smem, ok, 2);
     if (wpc == 3) return run(wpair_twin_kernel<8, 2, 0, 3>, smem, ok, 3);
     if (wpc == 6) return run(wpair_twin_kernel<8, 2, 0, 6>, smem, ok, 6);
+    if (cluster > 1 && csync == 1) return run(wpair_twin_kernel<8, 2, 0, 1, 1>, smem, ok, 1);
+    if (cluster > 1 && csync == 2) return run(wpair_twin_kernel<8, 2, 0, 1, 2>, smem, ok, 1);
     switch (hint) {
         case 1: return run(wpair_twin_kernel<8, 2, 1>, smem, ok, 1);
         case 2: return run(wpair_twin_kernel<8, 2, 2>, smem, ok, 1);
         case 3: return run(wpair_twin_kernel<8, 2, 3>, smem, ok, 1);
         default: return run(wpair_twin_kernel<8, 2, 0>, smem, ok, 1);
     }
+}
+
+// Launches the real fwd2d_wpair_kernel<8, *, *> on the same shapes (var as the library's WPAIR_VAR: 0 = <8, 2, 12>,
+// the db4 default; 1 = <8, 2, 15>; 3 = <8, 3, 12>) with taps dlo / dhi, as clusters of `cluster` strips at at most
+// ctas_per_sm CTAs per SM (0: as many as fit), so that it can be timed at the twin's settings.  Returns as
+// wpair_twin_fwd.
+extern "C" int wpair_kernel_fwd(int var, int ctas_per_sm, int cluster, const float* x, int64_t B, int H, int W,
+                                int64_t x_bs, int64_t x_rs, const wt_level* lv, int mode, const double* dlo,
+                                const double* dhi, void* stream) {
+    using namespace wtb;
+    WPairParams p;
+    CUtensorMap tmap;
+    int nstrip = 0;
+    Taps<float> taps;
+    for (int k = 0; k < 8; ++k) { taps.lo[k] = (float)dlo[k]; taps.hi[k] = (float)dhi[k]; }
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (var == 3) {
+        if (!wpair_plan<8, 3>(x, B, H, W, x_bs, x_rs, lv[0], lv[1], mode, taps, p, tmap, nstrip)) return -1;
+        return twin_launch(fwd2d_wpair_kernel<8, 3, 12>, p, tmap, nstrip, B,
+                           twin_smem((size_t)WPairGeom<8, 3>::SMEM, ctas_per_sm, 1), 1, cluster, st);
+    }
+    if (!wpair_plan<8, 2>(x, B, H, W, x_bs, x_rs, lv[0], lv[1], mode, taps, p, tmap, nstrip)) return -1;
+    const size_t smem = twin_smem((size_t)WPairGeom<8, 2>::SMEM, ctas_per_sm, 1);
+    if (var == 1) return twin_launch(fwd2d_wpair_kernel<8, 2, 15>, p, tmap, nstrip, B, smem, 1, cluster, st);
+    return twin_launch(fwd2d_wpair_kernel<8, 2, 12>, p, tmap, nstrip, B, smem, 1, cluster, st);
 }
