@@ -121,16 +121,20 @@ int wt_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * (general L: (n + padl + padr - L)/2 + 1 with the reference's pad amounts). */
 int64_t wt_coeff_len(int64_t n, int filt_len);
 
-/* Bytes of scratch wt_dwt_fwd / wt_dwt_inv need for the given problem (0 is possible: the fused kernels need
- * none).  inverse: 0 analysis, 1 synthesis; bit 1 set (2, 3) asks for the requirement of the GENERAL path whatever a
- * fused kernel covers -- a fused kernel can still decline at launch time (layouts it does not handle); the transform
- * then returns WT_EWORKSPACE and the caller retries with this amount. */
+/* Bytes of workspace wt_dwt_fwd / wt_dwt_inv need for the given problem, exactly: 0 when the call runs on the fused
+ * kernels, which need none, else the requirement of the general path.  Which of the two runs a call depends on its
+ * arguments here alone, so this query and the transform always agree.  inverse: 0 analysis, 1 synthesis; bit 1 is
+ * retired and ignored (2 and 3 give what 0 and 1 give).  dims are the extents of x (analysis) or of y (synthesis).
+ * Arguments the transform rejects give 0. */
 size_t wt_dwt_workspace_bytes(int ndim, int dtype, int levels, int filt_len, int64_t batch,
                               const int64_t* dims, int inverse);
 
 /* Multi-level analysis.  x is [batch, dims...] with element strides x_strides[ndim] and
  * batch stride x_batch_stride.  levels_desc[0] is the FINEST level (level 1),
- * levels_desc[levels-1] the coarsest.  mode: WT_MODE_*. */
+ * levels_desc[levels-1] the coarsest.  mode: WT_MODE_*.
+ * For ndim >= 2, x, every detail band and every approximation must have an innermost stride of 1 (WT_EINVAL).
+ * A call that returns WT_EINVAL, WT_ESHAPE or WT_EWORKSPACE (wt_dwt_inv alike) has launched nothing; only a CUDA
+ * error can come back after launches were made. */
 int wt_dwt_fwd(int ndim, int dtype, int mode, int levels, int filt_len,
                const double* dec_lo, const double* dec_hi,
                const void* x, int64_t batch, const int64_t* dims,

@@ -20,6 +20,7 @@
 // Algorithmic bytes per level: 4 B * (H*W read + 4*Mh*Mw written).
 #pragma once
 
+#include <cassert>
 #include <cuda.h>
 
 #include "common.cuh"
@@ -643,6 +644,26 @@ static bool make_tmap_3d(CUtensorMap* map, const T* base, int64_t B, int64_t H, 
     return r == CUDA_SUCCESS;
 }
 
+// Output columns per strip of the strip kernel: 64 in float32, 32 in float64.
+constexpr int fwd2d_strip_width(int es) { return es == 4 ? 64 : 32; }
+
+// Grid of a strip-kernel launch: nstrip strips (gridDim.x) by nseg segments of seg output rows (gridDim.y); the batch
+// rides on gridDim.z in launches of at most 65535 images.
+struct StripGrid { int nstrip, nseg, seg; };
+
+// Analysis level of Mh x Mw outputs per image, B images per launch.  Segments of 16 k - HALO/2 output rows keep the
+// chunking free of an idle tail; small levels get shorter ones so that the grid still fills the machine a few times
+// (fewer images never give fewer segments).
+static StripGrid fwd2d_grid(int64_t Mh, int64_t Mw, int64_t B, int L, int TW) {
+    const int HH = (L - 2) / 2;   // Fwd2dGeom::HALO / 2
+    const int64_t nstrip = (Mw + TW - 1) / TW;
+    int64_t nseg = (Mh + 255) / 256;
+    while (nseg * nstrip * B < 4 * 592 && (Mh + nseg - 1) / nseg > 48) ++nseg;
+    int64_t seg = ((Mh + nseg - 1) / nseg + HH + 15) / 16 * 16 - HH;
+    if (seg < 16 - HH) seg = 16 - HH;
+    return {(int)nstrip, (int)((Mh + seg - 1) / seg), (int)seg};
+}
+
 template <typename T, int L, int TW>
 static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64_t x_bs, int64_t x_rs, T* const out[4],
                                       const int64_t out_bs[4], const int64_t out_rs[4], int Mh, int Mw, int mode,
@@ -660,17 +681,9 @@ static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64
         if (((uintptr_t)out[k] & 15) || (out_bs[k] % VEC) || (out_rs[k] % VEC) || out_rs[k] < (Mw + VEC - 1) / VEC * VEC)
             p.vec_store = 0;
     }
-    // segments of 16 k - HALO/2 output rows so that the chunking has no idle tail
-    constexpr int HH = Gm::HALO / 2;
-    int nseg = (Mh + 255) / 256;
-    {   // small levels: shorter segments so that the grid still fills the machine a few times
-        const int64_t nstrip0 = (Mw + TW - 1) / TW;
-        while (nseg * nstrip0 * B < 4 * 592 && (Mh + nseg - 1) / nseg > 48) ++nseg;
-    }
-    int seg = ((Mh + nseg - 1) / nseg + HH + 15) / 16 * 16 - HH;
-    if (seg < 16 - HH) seg = 16 - HH;
-    nseg = (Mh + seg - 1) / seg;
-    p.seg_rows = seg;
+    const StripGrid g = fwd2d_grid(Mh, Mw, B, L, TW);
+    assert(g.nseg <= 65535 && "dwt_route sends levels whose segments overflow gridDim.y to the general path");
+    p.seg_rows = g.seg;
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     const bool tma = make_tmap_3d<T>(&tmap, x, B, H, W, x_bs, x_rs, Gm::SW, Gm::IN_ROWS);
@@ -692,11 +705,10 @@ static cudaError_t launch_fwd2d_level(const T* x, int64_t B, int H, int W, int64
     }
     cudaError_t e = ensure_dyn_smem(kern, smem);
     if (e != cudaSuccess) return e;
-    const int nstrip = (Mw + TW - 1) / TW;
     for (int64_t b0 = 0; b0 < B; b0 += 65535) {
         p.batch0 = (int)b0;
         const int nb = (int)((B - b0) < 65535 ? (B - b0) : 65535);
-        dim3 grid(nstrip, nseg, nb);
+        dim3 grid(g.nstrip, g.nseg, nb);
         kern<<<grid, Gm::NTHREADS, smem, st>>>(p, tmap);
         ++*launches;
         e = cudaGetLastError();
@@ -712,12 +724,6 @@ template <typename T>
 static bool try_fuse2(const T*, int64_t, int, int, int64_t, int64_t, const wt_level&, const wt_level&, int, int,
                       const Taps<T>&, cudaStream_t, uint64_t*, cudaError_t*);
 
-static bool fused2d_fwd_covers(int ndim, int L) {
-    return ndim == 2 && !(L & 1) && L <= 16 && !knob_on(K_DISABLE_FUSED);
-}
-
-// Try the fused path for the first levels of a 2-D analysis; *first_generic receives the number
-// of levels done here (the general path continues from there).
 // One auxiliary stream per device: the batch is cut into chunks that alternate between the caller's
 // stream and this one, so that the small, latency-bound launches of the deep levels of one chunk run
 // under the bandwidth-bound level-1 launch of the next (fork / join with events; no host sync).
@@ -746,17 +752,13 @@ static AuxStream* aux_stream_for_current_device() {
 }
 
 template <typename T>
-static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* dlo, const double* dhi, const T* x,
-                           int64_t batch, const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv,
-                           cudaStream_t st, int* first_generic);
+static int fused2d_fwd_run(int mode, int levels, int L, const double* dlo, const double* dhi, const T* x, int64_t batch,
+                           const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv, cudaStream_t st);
 
+// All levels of a 2-D analysis on the strip and level-pair kernels (dwt_route chose them).
 template <typename T>
-static int fused2d_fwd_try(int ndim, int mode, int levels, int L, const double* dlo, const double* dhi, const T* x,
-                           int64_t batch, const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv,
-                           cudaStream_t st, int* first_generic) {
-    *first_generic = 0;
-    if (!fused2d_fwd_covers(ndim, L)) return 0;
-    if (xs[1] != 1) return 0;
+static int fused2d_fwd(int mode, int levels, int L, const double* dlo, const double* dhi, const T* x, int64_t batch,
+                       const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv, cudaStream_t st) {
     // Chunking: the batch is cut into chunks that alternate between the caller's stream and one auxiliary
     // stream, so that the latency-bound deep levels of one chunk run under the bandwidth-bound level-1 launch
     // of the next.  The intermediate approximations cA_1 .. cA_{n-1} are scratch, so every chunk reuses the
@@ -774,13 +776,13 @@ static int fused2d_fwd_try(int ndim, int mode, int levels, int L, const double* 
     cudaStream_t s2 = aux ? aux->s : nullptr;
     if (!s2) nstreams = 1;
     if (chunk <= 0 || chunk >= batch || levels > 32)
-        return fused2d_fwd_run<T>(ndim, mode, levels, L, dlo, dhi, x, batch, dims, xs, xbs, lv, st, first_generic);
+        return fused2d_fwd_run<T>(mode, levels, L, dlo, dhi, x, batch, dims, xs, xbs, lv, st);
     if (nstreams > 1) {
         std::lock_guard<std::mutex> g(aux->mu);
         cudaEventRecord(aux->fork, st);
         cudaStreamWaitEvent(s2, aux->fork, 0);
     }
-    int rc = 0, fg = levels;
+    int rc = 0;
     wt_level sub[32];
     int c = 0;
     for (int64_t b0 = 0; b0 < batch && rc == 0; b0 += chunk, ++c) {
@@ -793,37 +795,19 @@ static int fused2d_fwd_try(int ndim, int mode, int levels, int L, const double* 
             // the last level's approximation is an output; the others are scratch (include/wtb200.h)
             sub[l].approx = (T*)lv[l].approx + (l == levels - 1 ? b0 : slot0) * lv[l].approx_batch_stride;
         }
-        int fgc = 0;
-        rc = fused2d_fwd_run<T>(ndim, mode, levels, L, dlo, dhi, x + b0 * xbs, b1 - b0, dims, xs, xbs, sub,
-                                which ? s2 : st, &fgc);
-        if (fgc < fg) fg = fgc;
-        if (c == 0 && rc == 0 && fgc < levels && b1 < batch) {
-            // the fused kernels stop before the last level (the general path continues on the whole batch and
-            // needs every item's approximation in place): no scratch reuse -- do the rest in one plain call
-            for (int l = 0; l < levels; ++l) {
-                sub[l] = lv[l];
-                sub[l].details = (T*)lv[l].details + b1 * lv[l].details_batch_stride;
-                sub[l].approx = (T*)lv[l].approx + b1 * lv[l].approx_batch_stride;
-            }
-            rc = fused2d_fwd_run<T>(ndim, mode, levels, L, dlo, dhi, x + b1 * xbs, batch - b1, dims, xs, xbs, sub, st, &fgc);
-            if (fgc < fg) fg = fgc;
-            break;
-        }
+        rc = fused2d_fwd_run<T>(mode, levels, L, dlo, dhi, x + b0 * xbs, b1 - b0, dims, xs, xbs, sub, which ? s2 : st);
     }
     if (nstreams > 1) {
         std::lock_guard<std::mutex> g(aux->mu);
         cudaEventRecord(aux->join, s2);
         cudaStreamWaitEvent(st, aux->join, 0);
     }
-    *first_generic = fg;
     return rc;
 }
 
 template <typename T>
-static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* dlo, const double* dhi, const T* x,
-                           int64_t batch, const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv,
-                           cudaStream_t st, int* first_generic) {
-    *first_generic = 0;
+static int fused2d_fwd_run(int mode, int levels, int L, const double* dlo, const double* dhi, const T* x, int64_t batch,
+                           const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv, cudaStream_t st) {
     Taps<T> taps;
     for (int k = 0; k < L; ++k) { taps.lo[k] = (T)dlo[k]; taps.hi[k] = (T)dhi[k]; }
     const T* src = x;
@@ -832,7 +816,6 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
     uint64_t launches = 0;
     for (int l = 0; l < levels; ++l) {
         const wt_level& d = lv[l];
-        if (H >= (1 << 30) || W >= (1 << 30)) break;
         if (l + 1 < levels) {
             // two levels in one launch, cA_{l+1} stays in shared memory: the kernel of independent warps
             // (fused2d_wpair.cuh) for levels 1-2 of images of >= WPAIR_MIN samples, at least 8 of them, else the
@@ -853,11 +836,9 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
                 src = (const T*)d2.approx; sbs = d2.approx_batch_stride; srs = d2.approx_strides[0];
                 H = d2.dims[0]; W = d2.dims[1];
                 ++l;
-                *first_generic = l + 1;
                 continue;
             }
         }
-        if (d.strides[1] != 1 || d.approx_strides[1] != 1) break;
         T* out[4];
         int64_t obs[4], ors[4];
         out[0] = (T*)d.approx; obs[0] = d.approx_batch_stride; ors[0] = d.approx_strides[0];
@@ -869,8 +850,8 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
         cudaError_t e = cudaSuccess;
 #define WTB_F2D_CASE(LL)                                                                                       \
     case LL:                                                                                                   \
-        e = launch_fwd2d_level<T, LL, (sizeof(T) == 4 ? 64 : 32)>(src, batch, (int)H, (int)W, sbs, srs, out, obs, ors, \
-                                                                  Mh, Mw, mode, taps, st, &launches);          \
+        e = launch_fwd2d_level<T, LL, fwd2d_strip_width(sizeof(T))>(src, batch, (int)H, (int)W, sbs, srs, out, obs,  \
+                                                                     ors, Mh, Mw, mode, taps, st, &launches);  \
         break;
         switch (L) {
             WTB_F2D_CASE(2)
@@ -887,7 +868,6 @@ static int fused2d_fwd_run(int ndim, int mode, int levels, int L, const double* 
         g_launches.fetch_add(launches, std::memory_order_relaxed);
         launches = 0;
         if (e != cudaSuccess) return cuda_fail(e, "fwd2d_strip_kernel");
-        *first_generic = l + 1;
         src = out[0]; sbs = obs[0]; srs = ors[0];
         H = Mh; W = Mw;
     }

@@ -287,29 +287,61 @@ static bool make_tmap_4d(CUtensorMap* map, const float* base, int64_t B, int64_t
                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static bool fused3d_fwd_covers(int ndim, int dtype_size, int L) {
-    return ndim == 3 && dtype_size == 4 && !(L & 1) && L >= 2 && L <= 8 && !knob_on(K_DISABLE_FUSED);
+// Grid of a 3-D tile-kernel launch: ntx x (nty * nseg) x B CTAs, segments of seg planes (analysis) or plane pairs
+// (synthesis).
+struct TileGrid3d {
+    int ntx, nty, nseg, seg;
+    bool fits(int64_t B) const { return (int64_t)nty * nseg <= 65535 && B <= 65535; }
+};
+
+// Output tiles (rows x columns) of fwd3d_tile_kernel.
+static const int FWD3D_TILES[3][2] = {{16, 32}, {11, 44}, {8, 64}};
+
+// Tile of an analysis level with Mh x Mw output planes: 16 x 32 unless another shape stages at least 25 % fewer input
+// elements per plane (narrow or short planes); FWD3D_TILE forces one.
+static int fwd3d_tile_shape(int64_t Mh, int64_t Mw, int L) {
+    int best = 0;
+    int64_t cost[3];
+    for (int c = 0; c < 3; ++c) {
+        const int th_ = FWD3D_TILES[c][0], tw_ = FWD3D_TILES[c][1];
+        cost[c] = ((Mh + th_ - 1) / th_) * ((Mw + tw_ - 1) / tw_) * (2 * th_ + L - 2) * (2 * tw_ + L - 2);
+    }
+    for (int c = 1; c < 3; ++c)
+        if (4 * cost[c] <= 3 * cost[0] && cost[c] < cost[best]) best = c;
+    if (knob_is_set(K_FWD3D_TILE)) {
+        const int forced = (int)knob_val(K_FWD3D_TILE, -1);
+        if (forced >= 0 && forced < 3) best = forced;
+    }
+    return best;
+}
+
+// Analysis level of Md x Mh x Mw outputs per volume: segments along depth only while the grid would not fill the
+// machine a few times.
+static TileGrid3d fwd3d_grid(int64_t Md, int64_t Mh, int64_t Mw, int64_t B, int TH, int TW) {
+    const int64_t ntx = (Mw + TW - 1) / TW, nty = (Mh + TH - 1) / TH;
+    int64_t nseg = 1;
+    while (nseg * ntx * nty * B < 4 * 296 && (Md + nseg - 1) / nseg > 24) ++nseg;
+    const int64_t seg = (Md + nseg - 1) / nseg;
+    return {(int)ntx, (int)nty, (int)((Md + seg - 1) / seg), (int)seg};
 }
 
 template <int L, int TH, int TW>
 static cudaError_t launch_fwd3d_tiles(Fwd3dParams& p, const float* x, int64_t B, int D, int H, int W, int64_t x_bs, int64_t x_ps,
-                                      int64_t x_rs, cudaStream_t st) {
+                                      int64_t x_rs, cudaStream_t st, uint64_t* launches) {
     using Gm = Fwd3dGeom<L, TH, TW>;
-    const int ntx = (p.Mw + TW - 1) / TW, nty = (p.Mh + TH - 1) / TH;
-    int nseg = 1;
-    while ((int64_t)nseg * ntx * nty * B < 4 * 296 && (p.Md + nseg - 1) / nseg > 24) ++nseg;
-    p.seg_planes = (p.Md + nseg - 1) / nseg;
-    nseg = (p.Md + p.seg_planes - 1) / p.seg_planes;
-    p.nty = nty;
-    if ((int64_t)nty * nseg > 65535 || B > 65535) return cudaErrorInvalidConfiguration;
+    const TileGrid3d g = fwd3d_grid(p.Md, p.Mh, p.Mw, B, TH, TW);
+    assert(g.fits(B) && "dwt_route sends levels whose tiles overflow the grid to the general path");
+    p.seg_planes = g.seg;
+    p.nty = g.nty;
     CUtensorMap tmap;
     memset(&tmap, 0, sizeof(tmap));
     const bool tma = make_tmap_4d(&tmap, x, B, D, H, W, x_bs, x_ps, x_rs, Gm::SW, Gm::ROWS);
     auto kern = tma ? fwd3d_tile_kernel<L, TH, TW, true> : fwd3d_tile_kernel<L, TH, TW, false>;
     cudaError_t e = ensure_dyn_smem(kern, (size_t)Gm::SMEM);
     if (e != cudaSuccess) return e;
-    dim3 grid(ntx, nty * nseg, (unsigned)B);
+    dim3 grid(g.ntx, g.nty * g.nseg, (unsigned)B);
     kern<<<grid, Gm::NT, Gm::SMEM, st>>>(p, tmap);
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -346,36 +378,16 @@ static cudaError_t launch_fwd3d_level(const float* x, int64_t B, int D, int H, i
         p.dl[j] = j < L ? p.bl[j] : make_float2(0.f, 0.f);
         p.dh[j] = j < L ? p.bh[j] : make_float2(0.f, 0.f);
     }
-    // tile shape: 16 x 32 unless another shape stages at least 25 % fewer input elements per plane
-    // (narrow or short planes)
-    static const int shapes[3][2] = {{16, 32}, {11, 44}, {8, 64}};
-    int best = 0;
-    int64_t cost[3];
-    for (int c = 0; c < 3; ++c) {
-        const int th_ = shapes[c][0], tw_ = shapes[c][1];
-        cost[c] = (int64_t)((p.Mh + th_ - 1) / th_) * ((p.Mw + tw_ - 1) / tw_) * (2 * th_ + L - 2) * (2 * tw_ + L - 2);
-    }
-    for (int c = 1; c < 3; ++c)
-        if (4 * cost[c] <= 3 * cost[0] && cost[c] < cost[best]) best = c;
-    if (knob_is_set(K_FWD3D_TILE)) {
-        const int forced = (int)knob_val(K_FWD3D_TILE, -1);
-        if (forced >= 0 && forced < 3) best = forced;
-    }
-    ++*launches;
-    switch (best) {
-        case 1: return launch_fwd3d_tiles<L, 11, 44>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st);
-        case 2: return launch_fwd3d_tiles<L, 8, 64>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st);
-        default: return launch_fwd3d_tiles<L, 16, 32>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st);
+    switch (fwd3d_tile_shape(p.Mh, p.Mw, L)) {
+        case 1: return launch_fwd3d_tiles<L, 11, 44>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st, launches);
+        case 2: return launch_fwd3d_tiles<L, 8, 64>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st, launches);
+        default: return launch_fwd3d_tiles<L, 16, 32>(p, x, B, D, H, W, x_bs, x_ps, x_rs, st, launches);
     }
 }
 
-// All levels of a float32 3-D analysis; *done = 1 when handled.
-static int fused3d_fwd_try(int mode, int levels, int L, const double* dlo, const double* dhi, const float* x, int64_t batch,
-                           const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv, cudaStream_t st, int* done) {
-    *done = 0;
-    if (xs[2] != 1 || batch > 65535) return 0;
-    for (int l = 0; l < levels; ++l)
-        if (lv[l].strides[2] != 1 || lv[l].approx_strides[2] != 1) return 0;
+// All levels of a float32 3-D analysis on the tile kernel (dwt_route chose it).
+static int fused3d_fwd(int mode, int levels, int L, const double* dlo, const double* dhi, const float* x, int64_t batch,
+                       const int64_t* dims, const int64_t* xs, int64_t xbs, const wt_level* lv, cudaStream_t st) {
     const float* src = x;
     int64_t sbs = xbs, sps = xs[0], srs = xs[1];
     int D = (int)dims[0], H = (int)dims[1], W = (int)dims[2];
@@ -395,7 +407,6 @@ static int fused3d_fwd_try(int mode, int levels, int L, const double* dlo, const
         src = (const float*)lv[l].approx; sbs = lv[l].approx_batch_stride; sps = lv[l].approx_strides[0]; srs = lv[l].approx_strides[1];
         D = (int)lv[l].dims[0]; H = (int)lv[l].dims[1]; W = (int)lv[l].dims[2];
     }
-    *done = 1;
     return 0;
 }
 

@@ -41,10 +41,12 @@ struct Inv2dMaps {
     CUtensorMap m[4];
 };
 
+constexpr int INV2D_TWO = 128;                                  // output columns per strip
+
 template <int L>
 struct Inv2dGeom {
     static constexpr int HALF = L / 2;
-    static constexpr int TWO = 128;                             // output columns per strip
+    static constexpr int TWO = INV2D_TWO;
     static constexpr int NC = TWO / 2 + HALF - 1;               // coefficient columns a strip reads
     static constexpr int CP = ((NC - 4 + 7) / 8) * 8 + 4;       // staged pitch, == 4 (mod 8), multiple of 4
     static constexpr int CR = 16;                               // coefficient rows per chunk
@@ -230,6 +232,18 @@ inv2d_strip_kernel(const __grid_constant__ Inv2dParams p, const __grid_constant_
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
+// Synthesis level of OH x OW outputs per image, B images per launch.  Segments of 32 k - 2 (HALF - 1) output rows keep
+// the chunking free of an idle tail; small levels get shorter ones so that the grid still fills the machine.
+static StripGrid inv2d_grid(int64_t OH, int64_t OW, int64_t B, int L) {
+    const int H1 = L / 2 - 1;   // Inv2dGeom::HALF - 1
+    const int64_t nstrip = (OW + INV2D_TWO - 1) / INV2D_TWO;
+    int64_t nseg = (OH + 511) / 512;
+    while (nseg * nstrip * B < 4 * 444 && (OH + nseg - 1) / nseg > 96) ++nseg;
+    int64_t seg = ((OH + nseg - 1) / nseg + 2 * H1 + 31) / 32 * 32 - 2 * H1;
+    if (seg < 2) seg = 2;
+    return {(int)nstrip, (int)((OH + seg - 1) / seg), (int)seg};
+}
+
 template <int L>
 static cudaError_t launch_inv2d_level(const float* const in[4], const int64_t in_bs[4], const int64_t in_rs[4], int64_t B,
                                       int Mh, int Mw, float* y, int64_t y_bs, int64_t y_rs, int OH, int OW,
@@ -251,21 +265,16 @@ static cudaError_t launch_inv2d_level(const float* const in[4], const int64_t in
         p.bh[k] = make_float2((float)rhi[k], (float)rhi[k]);
     }
     p.vec_store = !(((uintptr_t)y & 15) || (y_bs & 3) || (y_rs & 3) || y_rs < (OW + 3) / 4 * 4);
-    const int nstrip = (OW + Gm::TWO - 1) / Gm::TWO;
-    int nseg = (OH + 511) / 512;
-    while ((int64_t)nseg * nstrip * B < 4 * 444 && (OH + nseg - 1) / nseg > 96) ++nseg;
-    // segments of 32 k - 2 (HALF - 1) output rows keep the chunking free of an idle tail
-    int seg = ((OH + nseg - 1) / nseg + 2 * (Gm::HALF - 1) + 31) / 32 * 32 - 2 * (Gm::HALF - 1);
-    if (seg < 2) seg = 2;
-    nseg = (OH + seg - 1) / seg;
-    p.seg_rows = seg;
+    const StripGrid g = inv2d_grid(OH, OW, B, L);
+    assert(g.nseg <= 65535 && "dwt_route sends levels whose segments overflow gridDim.y to the general path");
+    p.seg_rows = g.seg;
     auto kern = tma ? inv2d_strip_kernel<L, true> : inv2d_strip_kernel<L, false>;
     cudaError_t e = ensure_dyn_smem(kern, (size_t)Gm::SMEM);
     if (e != cudaSuccess) return e;
     for (int64_t b0 = 0; b0 < B; b0 += 65535) {
         p.batch0 = (int)b0;
         const int nb = (int)((B - b0) < 65535 ? (B - b0) : 65535);
-        dim3 grid(nstrip, nseg, nb);
+        dim3 grid(g.nstrip, g.nseg, nb);
         kern<<<grid, Gm::NT, Gm::SMEM, st>>>(p, maps);
         ++*launches;
         e = cudaGetLastError();
@@ -274,19 +283,9 @@ static cudaError_t launch_inv2d_level(const float* const in[4], const int64_t in
     return cudaSuccess;
 }
 
-static bool fused2d_inv_covers(int ndim, int dtype_size, int L) {
-    return ndim == 2 && dtype_size == 4 && !(L & 1) && L >= 2 && L <= 16 && !knob_on(K_DISABLE_FUSED);
-}
-
-// All levels of a float32 2-D synthesis; returns 0 and sets *done = 1 when it handled the request.
-static int fused2d_inv_try(int levels, int L, const double* rlo, const double* rhi, float* y, int64_t batch,
-                           const int64_t* out_dims, const int64_t* ys, int64_t ybs, const wt_level* lv, cudaStream_t st,
-                           int* done) {
-    *done = 0;
-    if (ys[1] != 1) return 0;
-    for (int l = 0; l < levels; ++l)
-        if (lv[l].strides[1] != 1 || lv[l].approx_strides[1] != 1 || lv[l].dims[0] >= (1 << 30) || lv[l].dims[1] >= (1 << 30))
-            return 0;
+// All levels of a float32 2-D synthesis on the strip kernel (dwt_route chose it).
+static int fused2d_inv(int levels, int L, const double* rlo, const double* rhi, float* y, int64_t batch,
+                       const int64_t* out_dims, const int64_t* ys, int64_t ybs, const wt_level* lv, cudaStream_t st) {
     uint64_t launches = 0;
     for (int l = levels - 1; l >= 0; --l) {
         const wt_level& d = lv[l];
@@ -320,7 +319,6 @@ static int fused2d_inv_try(int levels, int L, const double* rlo, const double* r
         launches = 0;
         if (e != cudaSuccess) return cuda_fail(e, "inv2d_strip_kernel");
     }
-    *done = 1;
     return 0;
 }
 

@@ -35,10 +35,12 @@ struct Inv3dMaps {
     CUtensorMap m[8];
 };
 
+constexpr int INV3D_TOH = 16, INV3D_TOW = 64;                   // output tile
+
 template <int L>
 struct Inv3dGeom {
     static constexpr int HALF = L / 2;
-    static constexpr int TOH = 16, TOW = 64;                    // output tile
+    static constexpr int TOH = INV3D_TOH, TOW = INV3D_TOW;
     static constexpr int CRW = TOH / 2 + HALF - 1;              // coefficient rows per tile
     static constexpr int NCC = TOW / 2 + HALF - 1;              // coefficient columns per tile
     static constexpr int CP = ((NCC - 4 + 7) / 8) * 8 + 4;      // staged pitch (== 4 mod 8)
@@ -236,8 +238,14 @@ inv3d_tile_kernel(const __grid_constant__ Inv3dParams p, const __grid_constant__
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-static bool fused3d_inv_covers(int ndim, int dtype_size, int L) {
-    return ndim == 3 && dtype_size == 4 && !(L & 1) && L >= 2 && L <= 8 && !knob_on(K_DISABLE_FUSED);
+// Synthesis level of OD x OH x OW outputs per volume: segments along depth only while the grid would not fill the
+// machine a few times.
+static TileGrid3d inv3d_grid(int64_t OD, int64_t OH, int64_t OW, int64_t B) {
+    const int64_t ntx = (OW + INV3D_TOW - 1) / INV3D_TOW, nty = (OH + INV3D_TOH - 1) / INV3D_TOH, npairs = (OD + 1) / 2;
+    int64_t nseg = 1;
+    while (nseg * ntx * nty * B < 4 * 296 && (npairs + nseg - 1) / nseg > 16) ++nseg;
+    const int64_t seg = (npairs + nseg - 1) / nseg;
+    return {(int)ntx, (int)nty, (int)((npairs + seg - 1) / seg), (int)seg};
 }
 
 template <int L>
@@ -266,29 +274,22 @@ static cudaError_t launch_inv3d_level(const wt_level& d, int64_t B, float* y, in
         p.bh[k] = make_float2((float)rhi[k], (float)rhi[k]);
     }
     p.vec_store = !(((uintptr_t)y & 15) || (y_bs & 3) || (y_ps & 3) || (y_rs & 3) || y_rs < (OW + 3) / 4 * 4);
-    const int ntx = (OW + Gm::TOW - 1) / Gm::TOW, nty = (OH + Gm::TOH - 1) / Gm::TOH;
-    const int npairs = (OD + 1) / 2;
-    int nseg = 1;
-    while ((int64_t)nseg * ntx * nty * B < 4 * 296 && (npairs + nseg - 1) / nseg > 16) ++nseg;
-    p.seg_pairs = (npairs + nseg - 1) / nseg;
-    nseg = (npairs + p.seg_pairs - 1) / p.seg_pairs;
-    p.nty = nty;
-    if ((int64_t)nty * nseg > 65535 || B > 65535) return cudaErrorInvalidConfiguration;
+    const TileGrid3d g = inv3d_grid(OD, OH, OW, B);
+    assert(g.fits(B) && "dwt_route sends levels whose tiles overflow the grid to the general path");
+    p.seg_pairs = g.seg;
+    p.nty = g.nty;
     auto kern = tma ? inv3d_tile_kernel<L, true> : inv3d_tile_kernel<L, false>;
     cudaError_t e = ensure_dyn_smem(kern, (size_t)Gm::SMEM);
     if (e != cudaSuccess) return e;
-    dim3 grid(ntx, nty * nseg, (unsigned)B);
+    dim3 grid(g.ntx, g.nty * g.nseg, (unsigned)B);
     kern<<<grid, Gm::NT, Gm::SMEM, st>>>(p, maps);
     ++*launches;
     return cudaGetLastError();
 }
 
-static int fused3d_inv_try(int levels, int L, const double* rlo, const double* rhi, float* y, int64_t batch,
-                           const int64_t* out_dims, const int64_t* ys, int64_t ybs, const wt_level* lv, cudaStream_t st, int* done) {
-    *done = 0;
-    if (ys[2] != 1 || batch > 65535) return 0;
-    for (int l = 0; l < levels; ++l)
-        if (lv[l].strides[2] != 1 || lv[l].approx_strides[2] != 1) return 0;
+// All levels of a float32 3-D synthesis on the tile kernel (dwt_route chose it).
+static int fused3d_inv(int levels, int L, const double* rlo, const double* rhi, float* y, int64_t batch,
+                       const int64_t* out_dims, const int64_t* ys, int64_t ybs, const wt_level* lv, cudaStream_t st) {
     uint64_t launches = 0;
     for (int l = levels - 1; l >= 0; --l) {
         float* dst; int64_t dbs, dps, drs; int OD, OH, OW;
@@ -310,7 +311,6 @@ static int fused3d_inv_try(int levels, int L, const double* rlo, const double* r
         launches = 0;
         if (e != cudaSuccess) return cuda_fail(e, "inv3d_tile_kernel");
     }
-    *done = 1;
     return 0;
 }
 

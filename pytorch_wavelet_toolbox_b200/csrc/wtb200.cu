@@ -162,21 +162,67 @@ static void generic_scratch_elems(int ndim, int L, int levels, int64_t batch, co
     }
 }
 
+// Which kernels run a 2-D or 3-D DWT call: the fused kernels, which run every level and need no workspace, or the
+// general path (dwt_fwd_generic / dwt_inv_generic), which needs generic_scratch_elems.  Decided from the call's shapes
+// alone, before its first launch, for wt_dwt_workspace_bytes and the transform alike, so the two always agree and a
+// fused call never falls through to the general path.  The limits are those of the launchers, computed by the same
+// geometry functions.  dims are the input extents of an analysis, the output extents of a synthesis.
+enum DwtRoute { ROUTE_GENERAL, ROUTE_FUSED2D, ROUTE_FUSED3D };
+
+static DwtRoute dwt_route(bool inverse, int ndim, int es, int levels, int L, int64_t batch, const int64_t* dims) {
+    if (ndim < 2 || (L & 1) || knob_on(K_DISABLE_FUSED)) return ROUTE_GENERAL;
+    if (ndim == 2 && (L > 16 || (inverse && es != 4))) return ROUTE_GENERAL;
+    if (ndim == 3 && (L > 8 || es != 4 || batch > 65535)) return ROUTE_GENERAL;   // 3-D: the batch is gridDim.z
+    // per level: n[] its input (analysis) or output (synthesis) extents, m[] its coefficient extents (coeff_len is
+    // exact in both directions for even L)
+    int64_t n[3], m[3];
+    for (int a = 0; a < ndim; ++a) n[a] = dims[a];
+    for (int l = 0; l < levels; ++l) {
+        for (int a = 0; a < ndim; ++a) {
+            m[a] = coeff_len(n[a], L);
+            // 2-D: the strip kernels take level inputs (analysis) or coefficients (synthesis) below 2^30;
+            // 3-D: the tile launchers narrow every extent to int
+            if (ndim == 2 ? (inverse ? m[a] : n[a]) >= (int64_t(1) << 30) : n[a] >= (int64_t(1) << 31))
+                return ROUTE_GENERAL;
+        }
+        bool fits;
+        if (ndim == 2 && !inverse) {
+            // the level-pair kernels fall back to the strip kernel, so it has to fit every level; a chunk of the
+            // batch may be one image, which gives the most segments
+            fits = fwd2d_grid(m[0], m[1], 1, L, fwd2d_strip_width(es)).nseg <= 65535;
+        } else if (ndim == 2) {
+            fits = inv2d_grid(n[0], n[1], batch, L).nseg <= 65535;
+        } else if (!inverse) {
+            const int* tile = FWD3D_TILES[fwd3d_tile_shape(m[1], m[2], L)];
+            fits = fwd3d_grid(m[0], m[1], m[2], batch, tile[0], tile[1]).fits(batch);
+        } else {
+            fits = inv3d_grid(n[0], n[1], n[2], batch).fits(batch);
+        }
+        if (!fits) return ROUTE_GENERAL;
+        for (int a = 0; a < ndim; ++a) n[a] = m[a];
+    }
+    return ndim == 2 ? ROUTE_FUSED2D : ROUTE_FUSED3D;
+}
+
+// The kernels of both paths read and write rows of unit stride.
+static bool unit_rows(int ndim, const int64_t* strides, const wt_level* lv, int levels) {
+    const int a = ndim - 1;
+    if (strides[a] != 1) return false;
+    for (int l = 0; l < levels; ++l)
+        if (lv[l].strides[a] != 1 || lv[l].approx_strides[a] != 1) return false;
+    return true;
+}
+
 template <typename T>
 static int dwt_fwd_generic(int ndim, int mode, int levels, int L, const Taps<T>& taps, const T* x,
                            int64_t batch, const int64_t* dims, const int64_t* xs, int64_t xbs,
-                           const wt_level* lv, int first_level, T* ws, cudaStream_t st) {
+                           const wt_level* lv, T* ws, cudaStream_t st) {
     int64_t cur[3];
     int64_t cs[3];
     int64_t cbs = xbs;
     const T* src = x;
     for (int a = 0; a < ndim; ++a) { cur[a] = dims[a]; cs[a] = xs[a]; }
-    for (int l = 0; l < first_level; ++l) {
-        // skip levels already done by a specialised kernel
-        src = (const T*)lv[l].approx; cbs = lv[l].approx_batch_stride;
-        for (int a = 0; a < ndim; ++a) { cur[a] = lv[l].dims[a]; cs[a] = lv[l].approx_strides[a]; }
-    }
-    for (int l = first_level; l < levels; ++l) {
+    for (int l = 0; l < levels; ++l) {
         if (ndim == 1 && cs[0] == 1 && !knob_on(K_DISABLE_FUSED)) {
             // group of consecutive levels -> one fused launch (intermediate approximations stay in shared memory;
             // their scratch buffers are left untouched, see the scratch semantics in include/wtb200.h)
@@ -245,7 +291,6 @@ static int dwt_fwd_generic(int ndim, int mode, int levels, int L, const Taps<T>&
             T* tlo = ws;
             T* thi = ws + batch * H * Mw;
             // pass along W (last axis): [batch, H, W] -> t{lo,hi} [batch, H, Mw]
-            if (cs[1] != 1) return fail(WT_EINVAL, "innermost stride must be 1");
             {
                 View<const T> xv{src, cbs, cs[0], 1};
                 View<T> lo{tlo, H * Mw, Mw, 1}, hi{thi, H * Mw, Mw, 1};
@@ -257,15 +302,12 @@ static int dwt_fwd_generic(int ndim, int mode, int levels, int L, const Taps<T>&
                 View<const T> xv{w ? thi : tlo, H * Mw, 0, Mw};
                 View<T> lo = band(w), hi = band(2 + w);
                 lo.s_n = st_of(w)[0]; hi.s_n = st_of(2 + w)[0];
-                if (st_of(w)[1] != 1 || st_of(2 + w)[1] != 1) return fail(WT_EINVAL, "innermost stride must be 1");
                 e = launch_axis_fwd<T>(xv, lo, hi, batch, 1, H, Mw, mode, L, taps, st);
                 if (e != cudaSuccess) return cuda_fail(e, "axis_fwd_kernel(H)");
             }
         } else {
             const int64_t D = cur[0], H = cur[1], W = cur[2];
             const int64_t Mh = d.dims[1], Mw = d.dims[2];
-            if (cs[2] != 1 || d.strides[2] != 1 || d.approx_strides[2] != 1)
-                return fail(WT_EINVAL, "innermost stride must be 1");
             const int64_t n1 = batch * D * H * Mw;
             T* t1[2] = {ws, ws + n1};
             const int64_t n2 = batch * D * Mh * Mw;
@@ -315,9 +357,8 @@ static int dwt_fwd_generic(int ndim, int mode, int levels, int L, const Taps<T>&
 template <typename T>
 static int dwt_inv_generic(int ndim, int levels, int L, const Taps<T>& taps, T* y, int64_t batch,
                            const int64_t* out_dims, const int64_t* ys, int64_t ybs, const wt_level* lv,
-                           int last_level, T* ws, cudaStream_t st) {
-    // last_level: levels [levels-1 .. last_level] are processed here (last_level = 0 -> all)
-    for (int l = levels - 1; l >= last_level; --l) {
+                           T* ws, cudaStream_t st) {
+    for (int l = levels - 1; l >= 0; --l) {
         const wt_level& d = lv[l];
         const T* det = (const T*)d.details;
         const T* app = (const T*)d.approx;
@@ -356,8 +397,6 @@ static int dwt_inv_generic(int ndim, int levels, int L, const Taps<T>& taps, T* 
             if (e != cudaSuccess) return cuda_fail(e, "axis_inv_kernel");
         } else if (ndim == 2) {
             const int64_t Mh = d.dims[0], Mw = d.dims[1], OH = dd[0], OW = dd[1];
-            if (d.strides[1] != 1 || d.approx_strides[1] != 1 || ds[1] != 1)
-                return fail(WT_EINVAL, "innermost stride must be 1");
             T* t[2] = {ws, ws + batch * OH * Mw};
             // along H: (k=0,k=2) -> t_lo ; (k=1,k=3) -> t_hi    [batch, OH, Mw]
             for (int w = 0; w < 2; ++w) {
@@ -375,8 +414,6 @@ static int dwt_inv_generic(int ndim, int levels, int L, const Taps<T>& taps, T* 
         } else {
             const int64_t Md = d.dims[0], Mh = d.dims[1], Mw = d.dims[2];
             const int64_t OD = dd[0], OH = dd[1], OW = dd[2];
-            if (d.strides[2] != 1 || d.approx_strides[2] != 1 || ds[2] != 1)
-                return fail(WT_EINVAL, "innermost stride must be 1");
             const int64_t n1 = batch * OD * Mh * Mw;
             T* t1 = ws;                 // 4 arrays [batch, OD, Mh, Mw]
             T* t2 = ws + 4 * n1;        // 2 arrays [batch, OD, OH, Mw]
@@ -444,28 +481,17 @@ static int dwt_fwd_t(int ndim, int mode, int levels, int L, const double* dlo, c
         }
         if (!lv[l].details || !lv[l].approx) return fail(WT_EINVAL, "level %d: NULL buffer", l + 1);
     }
+    if (ndim > 1 && !unit_rows(ndim, xs, lv, levels)) return fail(WT_EINVAL, "innermost stride must be 1");
+    const DwtRoute route = dwt_route(false, ndim, sizeof(T), levels, L, batch, dims);
+    if constexpr (sizeof(T) == 4) {
+        if (route == ROUTE_FUSED3D) return fused3d_fwd(mode, levels, L, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, st);
+    }
+    if (route == ROUTE_FUSED2D) return fused2d_fwd<T>(mode, levels, L, dlo, dhi, (const T*)x, batch, dims, xs, xbs, lv, st);
     int64_t s1, s2;
     generic_scratch_elems(ndim, L, levels, batch, dims, 0, &s1, &s2);
-    int first_generic = 0;
-    if constexpr (sizeof(T) == 4) {
-        if (fused3d_fwd_covers(ndim, 4, L)) {
-            int done = 0;
-            int rc = fused3d_fwd_try(mode, levels, L, dlo, dhi, (const float*)x, batch, dims, xs, xbs, lv, st, &done);
-            if (rc != 0 || done) return rc;
-        }
-    }
-    {
-        int rc = fused2d_fwd_try<T>(ndim, mode, levels, L, dlo, dhi, (const T*)x, batch, dims, xs, xbs, lv,
-                                    st, &first_generic);
-        if (rc != 0) return rc;
-    }
-    if (first_generic < levels) {
-        if (ndim > 1 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
-            return fail(WT_EWORKSPACE, "workspace: need %zu bytes, have %zu", (size_t)(s1 + s2) * sizeof(T), ws_bytes);
-        return dwt_fwd_generic<T>(ndim, mode, levels, L, taps, (const T*)x, batch, dims, xs, xbs, lv,
-                                  first_generic, (T*)ws, st);
-    }
-    return 0;
+    if (ndim > 1 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
+        return fail(WT_EWORKSPACE, "workspace: need %zu bytes, have %zu", (size_t)(s1 + s2) * sizeof(T), ws_bytes);
+    return dwt_fwd_generic<T>(ndim, mode, levels, L, taps, (const T*)x, batch, dims, xs, xbs, lv, (T*)ws, st);
 }
 
 template <typename T>
@@ -485,23 +511,17 @@ static int dwt_inv_t(int ndim, int levels, int L, const double* rlo, const doubl
         }
         if (!lv[l].details || !lv[l].approx) return fail(WT_EINVAL, "level %d: NULL buffer", l + 1);
     }
+    if (ndim > 1 && !unit_rows(ndim, ys, lv, levels)) return fail(WT_EINVAL, "innermost stride must be 1");
+    const DwtRoute route = dwt_route(true, ndim, sizeof(T), levels, L, batch, out_dims);
     if constexpr (sizeof(T) == 4) {
-        if (fused2d_inv_covers(ndim, 4, L)) {
-            int done = 0;
-            int rc = fused2d_inv_try(levels, L, rlo, rhi, (float*)y, batch, out_dims, ys, ybs, lv, st, &done);
-            if (rc != 0 || done) return rc;
-        }
-        if (fused3d_inv_covers(ndim, 4, L)) {
-            int done = 0;
-            int rc = fused3d_inv_try(levels, L, rlo, rhi, (float*)y, batch, out_dims, ys, ybs, lv, st, &done);
-            if (rc != 0 || done) return rc;
-        }
+        if (route == ROUTE_FUSED2D) return fused2d_inv(levels, L, rlo, rhi, (float*)y, batch, out_dims, ys, ybs, lv, st);
+        if (route == ROUTE_FUSED3D) return fused3d_inv(levels, L, rlo, rhi, (float*)y, batch, out_dims, ys, ybs, lv, st);
     }
     int64_t s1, s2;
     generic_scratch_elems(ndim, L, levels, batch, out_dims, 1, &s1, &s2);
-    if (ndim > 1 && levels > 0 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
+    if (ndim > 1 && ((size_t)(s1 + s2) * sizeof(T) > ws_bytes || !ws))
         return fail(WT_EWORKSPACE, "workspace: need %zu bytes, have %zu", (size_t)(s1 + s2) * sizeof(T), ws_bytes);
-    return dwt_inv_generic<T>(ndim, levels, L, taps, (T*)y, batch, out_dims, ys, ybs, lv, 0, (T*)ws, st);
+    return dwt_inv_generic<T>(ndim, levels, L, taps, (T*)y, batch, out_dims, ys, ybs, lv, (T*)ws, st);
 }
 
 // ---- matrix FWT -------------------------------------------------------------------------
@@ -1136,22 +1156,13 @@ int64_t wt_coeff_len(int64_t n, int filt_len) { return coeff_len(n, filt_len); }
 
 size_t wt_dwt_workspace_bytes(int ndim, int dtype, int levels, int filt_len, int64_t batch, const int64_t* dims,
                               int inverse) {
-    if (ndim < 1 || ndim > 3 || !dims || levels <= 0) return 0;
-    const bool general = (inverse & 2) != 0;   // bit 1: the requirement of the general path, whatever a fused path covers
-    inverse &= 1;
-    if (general) {
-        // fall through to the general requirement
-    } else if (!inverse && fused2d_fwd_covers(ndim, filt_len)) {
-        // the fused path needs no scratch unless it has to bail out (odd strides); keep the
-        // general path's requirement only when the fused path is disabled
-        return 0;
-    }
-    else if (inverse && fused2d_inv_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len)) return 0;
-    else if (!inverse && fused3d_fwd_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len) && batch <= 65535) return 0;
-    else if (inverse && fused3d_inv_covers(ndim, dtype == WT_F64 ? 8 : 4, filt_len) && batch <= 65535) return 0;
+    if (check_common(ndim, dtype, levels, filt_len, batch, dims) || levels == 0 || batch == 0) return 0;
+    inverse &= 1;   // bit 1 is retired (include/wtb200.h)
+    const int es = dtype == WT_F64 ? 8 : 4;
+    if (dwt_route(inverse, ndim, es, levels, filt_len, batch, dims) != ROUTE_GENERAL) return 0;
     int64_t s1, s2;
     generic_scratch_elems(ndim, filt_len, levels, batch, dims, inverse, &s1, &s2);
-    return (size_t)(s1 + s2) * (dtype == WT_F64 ? 8 : 4);
+    return (size_t)(s1 + s2) * es;
 }
 
 int wt_dwt_fwd(int ndim, int dtype, int mode, int levels, int filt_len, const double* dec_lo,

@@ -425,16 +425,13 @@ def _run_fwd(xd: torch.Tensor, plan: _Plan, mode: str, dec_lo, dec_hi, buf: torc
     levels = _fill_levels(plan, buf, scratch)
     code = _dtype_code(dt)
     stream = torch.cuda.current_stream(xd.device).cuda_stream
-    for general in (0, 2):
-        ws_bytes = int(lib.wt_dwt_workspace_bytes(plan.ndim, code, len(plan.levels), plan.filt_len, batch, dims_p, general))
-        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=xd.device) if ws_bytes else None
-        rc = lib.wt_dwt_fwd(
-            plan.ndim, code, N.MODES[mode], len(plan.levels), plan.filt_len, lo_p, hi_p,
-            xd.data_ptr(), batch, dims_p, xs_p, xd.stride(0), levels,
-            ws.data_ptr() if ws is not None else None, ws_bytes, stream,
-        )
-        if rc != N.WT_EWORKSPACE:
-            break   # a fused kernel declined at launch time: once more with the general path's scratch
+    ws_bytes = int(lib.wt_dwt_workspace_bytes(plan.ndim, code, len(plan.levels), plan.filt_len, batch, dims_p, 0))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=xd.device) if ws_bytes else None
+    rc = lib.wt_dwt_fwd(
+        plan.ndim, code, N.MODES[mode], len(plan.levels), plan.filt_len, lo_p, hi_p,
+        xd.data_ptr(), batch, dims_p, xs_p, xd.stride(0), levels,
+        ws.data_ptr() if ws is not None else None, ws_bytes, stream,
+    )
     N.check(rc, "wt_dwt_fwd")
 
 
@@ -594,13 +591,10 @@ def _synthesis(approx: torch.Tensor, levels_in: list[list[torch.Tensor]], probes
         ys_arr, ys_p = N.i64_array(y.stride()[1:])
         code = _dtype_code(dt)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        for general in (1, 3):
-            ws_bytes = int(lib.wt_dwt_workspace_bytes(ndim, code, nl, filt_len, batch, od_p, general))
-            ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev) if ws_bytes else None
-            rc = lib.wt_dwt_inv(ndim, code, nl, filt_len, lo_p, hi_p, y.data_ptr(), batch, od_p, ys_p, y.stride(0),
-                                arr, ws.data_ptr() if ws is not None else None, ws_bytes, stream)
-            if rc != N.WT_EWORKSPACE:
-                break   # a fused kernel declined at launch time: once more with the general path's scratch
+        ws_bytes = int(lib.wt_dwt_workspace_bytes(ndim, code, nl, filt_len, batch, od_p, 1))
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
+        rc = lib.wt_dwt_inv(ndim, code, nl, filt_len, lo_p, hi_p, y.data_ptr(), batch, od_p, ys_p, y.stride(0),
+                            arr, ws.data_ptr() if ws is not None else None, ws_bytes, stream)
         N.check(rc, "wt_dwt_inv")
         if on_host:
             host = pinned_empty(y.shape, dt)
