@@ -25,7 +25,7 @@ from .fwt import host_staging, wavedec, wavedec2, wavedec3, waverec, waverec2, w
 from .matrix_fwt import MatrixWavedec, MatrixWaverec, construct_boundary_a, construct_boundary_s
 from .matrix_fwt_nd import MatrixWavedec2, MatrixWavedec3, MatrixWaverec2, MatrixWaverec3
 from .separable import fswavedec2, fswavedec3, fswaverec2, fswaverec3
-from .packets import WaveletPacket, WaveletPacket2D
+from .packets import WaveletPacket, WaveletPacket2D, WaveletPacket3D
 from .stationary import iswt, swt
 from .continuous import cwt
 
@@ -43,7 +43,10 @@ NEXT_ROW_NAMES = (
     "cwt",                                                                   # continuous transform, csrc/cwt.cuh
 )
 
-__all__ = list(HOT_PATH_NAMES) + list(NEXT_ROW_NAMES) + [
+#: additions beyond the ptwt API: ptwt has no such names, so install() has nothing to rebind for them
+BEYOND_PTWT_NAMES = ("WaveletPacket3D",)
+
+__all__ = list(HOT_PATH_NAMES) + list(NEXT_ROW_NAMES) + list(BEYOND_PTWT_NAMES) + [
     "Wavelet", "WaveletTensorTuple", "WaveletDetailTuple2d", "WaveletDetailDict", "WaveletCoeff1d",
     "WaveletCoeff2d", "WaveletCoeffNd", "construct_boundary_a", "construct_boundary_s", "install", "uninstall", "host_staging",
 ]

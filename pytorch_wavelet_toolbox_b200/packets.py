@@ -11,6 +11,10 @@ tree level instead of one per node); ``reconstruct`` runs one synthesis call per
 The reference's quirk in separable mode is kept: ``fsdict["ad"] -> horizontal, fsdict["da"] -> vertical``
 (``packets.py:603-606``), although ``"ad"`` (low-pass on axis -2, high-pass on axis -1) is the VERTICAL band of
 ``wavedec2`` (SURVEY.md appendix A, quirk 10).
+
+``WaveletPacket3D`` goes beyond the ``ptwt`` API, which stops at 2-D packets: the same semantics for volumes and clips,
+one level-1 ``wavedec3`` / ``fswavedec3`` / ``MatrixWavedec3`` call on the stacked parents per tree level.  A node key
+is one 3-letter subband key (``wavedec3``'s ``"aad"`` .. ``"ddd"`` plus ``"aaa"``) per level.
 """
 from __future__ import annotations
 
@@ -23,12 +27,15 @@ import torch
 from ._shape import ensure_axes
 from ._wavelets import as_wavelet, dwt_max_level
 from .constants import WaveletDetailTuple2d
-from .fwt import wavedec, wavedec2, waverec, waverec2
+from .fwt import wavedec, wavedec2, wavedec3, waverec, waverec2, waverec3
 from .matrix_fwt import MatrixWavedec, MatrixWaverec, _ORTH_METHODS
-from .matrix_fwt_nd import MatrixWavedec2, MatrixWaverec2
-from .separable import fswavedec2, fswaverec2
+from .matrix_fwt_nd import MatrixWavedec2, MatrixWavedec3, MatrixWaverec2, MatrixWaverec3
+from .separable import fswavedec2, fswavedec3, fswaverec2, fswaverec3
 
-__all__ = ["WaveletPacket", "WaveletPacket2D"]
+__all__ = ["WaveletPacket", "WaveletPacket2D", "WaveletPacket3D"]
+
+#: the eight children of a 3-D packet node in natural order; letter i is the filter along axes[i]
+SUBBANDS_3D = tuple("".join(p) for p in product("ad", repeat=3))
 
 
 def _graycode_order(level: int, x: str = "a", y: str = "d") -> list[str]:
@@ -47,23 +54,33 @@ def _neg_axes(axes: Sequence[int], ndim: int) -> tuple[int, ...]:
 
 
 class _PacketBase(collections.UserDict):
-    _filter_keys: frozenset = frozenset()
+    _filter_keys: frozenset = frozenset()   # a node's children, as suffixes of its key
+    _key_chars: frozenset = frozenset()     # the letters a key may contain
+    _key_width = 1                          # letters per tree level
     _ndim = 1
+
+    def _invalid_key(self, key: str) -> ValueError:
+        rule = f"All chars in the key must be of the set {set(self._key_chars)}."
+        if self._key_width > 1:
+            rule += f" Its length must be a multiple of {self._key_width}, one subband key per level."
+        return ValueError(f"Invalid key '{key}'. {rule}")
 
     def _check_access(self, key: str) -> None:
         """The reference's access checks (packets.py:332-359, 642-665), in its order."""
         if self.maxlevel is None:
             raise ValueError("The wavelet packet tree must be initialized via 'transform' before "
                              "its values can be accessed!")
-        if key not in self and len(key) > self.maxlevel:
-            raise KeyError(f"The requested level {len(key)} with key '{key}' is too large and cannot be accessed! "
+        w = self._key_width
+        level = -(-len(key) // w)
+        if key not in self and level > self.maxlevel:
+            raise KeyError(f"The requested level {level} with key '{key}' is too large and cannot be accessed! "
                            f"This wavelet packet tree is initialized with maximum level {self.maxlevel}.")
         if key not in self:
             if key == "":
                 raise ValueError("The requested root of the packet tree cannot be accessed! The wavelet packet tree is "
                                  "not properly initialized. Run `transform` before accessing tree values.")
-            if key[-1] not in self._filter_keys:
-                raise ValueError(f"Invalid key '{key}'. All chars in the key must be of the set {set(self._filter_keys)}.")
+            if len(key) % w or key[-w:] not in self._filter_keys:
+                raise self._invalid_key(key)
 
     def __getitem__(self, key: str) -> torch.Tensor:
         self._check_access(key)
@@ -81,18 +98,20 @@ class _PacketBase(collections.UserDict):
         self._require(keys)
 
     def _require(self, keys: Sequence[str]) -> None:
-        depth = max((len(k) for k in keys), default=0)
+        w = self._key_width
+        depth = max((len(k) // w for k in keys), default=0)
         for level in range(depth):
+            start = level * w
             parents: list[str] = []
             for k in keys:
-                if len(k) > level and k not in self.data:
-                    par = k[:level]
+                if len(k) > start and k not in self.data:
+                    par = k[:start]
                     if par not in parents and not self._expanded(par):
                         parents.append(par)
             # validate the requests of this level like a node-by-node walk would
             for k in keys:
-                if len(k) > level and k[level] not in self._filter_keys:
-                    raise ValueError(f"Invalid key '{k}'. All chars in the key must be of the set {set(self._filter_keys)}.")
+                if len(k) > start and k[start:start + w] not in self._filter_keys:
+                    raise self._invalid_key(k)
             if parents:
                 self._expand_nodes(parents)
 
@@ -108,6 +127,7 @@ class WaveletPacket(_PacketBase):
     """One-dimensional wavelet packets (reference packets.py:68-360), level-wise batched."""
 
     _filter_keys = frozenset({"a", "d"})
+    _key_chars = _filter_keys
 
     def __init__(self, data: Optional[torch.Tensor], wavelet: Any, *, mode: str = "reflect",
                  maxlevel: Optional[int] = None, axis: Optional[int] = None, orthogonalization: str = "qr",
@@ -207,6 +227,7 @@ class WaveletPacket2D(_PacketBase):
     """Two-dimensional wavelet packets (reference packets.py:362-771), level-wise batched."""
 
     _filter_keys = frozenset({"a", "h", "v", "d"})
+    _key_chars = _filter_keys
     _ndim = 2
 
     def __init__(self, data: Optional[torch.Tensor], wavelet: Any, *, mode: str = "reflect",
@@ -329,3 +350,142 @@ class WaveletPacket2D(_PacketBase):
             grid.setdefault(row, {})[col] = "".join(node)
         order = _graycode_order(level, x="l", y="h") if level > 0 else ["l", "h"]
         return [[grid[r][c] for c in order if c in grid[r]] for r in order if r in grid]
+
+
+class WaveletPacket3D(_PacketBase):
+    """Three-dimensional wavelet packets, level-wise batched (an addition beyond the ``ptwt`` API).
+
+    Every node is one level-1 ``wavedec3`` of its parent (``fswavedec3`` with ``separable=True``, ``MatrixWavedec3``
+    in mode ``"boundary"``); its key appends the subband key (``"aaa"`` .. ``"ddd"``, first letter along ``axes[0]``)
+    to the parent's, so ``"aad"`` lies at depth 1 and ``"aaddda"`` at depth 2.
+    """
+
+    _filter_keys = frozenset(SUBBANDS_3D)
+    _key_chars = frozenset({"a", "d"})
+    _key_width = 3
+    _ndim = 3
+
+    def __init__(self, data: Optional[torch.Tensor], wavelet: Any, *, mode: str = "reflect",
+                 maxlevel: Optional[int] = None, axes: tuple[int, int, int] = (-3, -2, -1),
+                 orthogonalization: str = "qr", separable: bool = False, **deprecated: Any) -> None:
+        if "boundary_orthogonalization" in deprecated:
+            import warnings
+
+            warnings.warn("boundary_orthogonalization is deprecated; use orthogonalization", DeprecationWarning, stacklevel=2)
+            orthogonalization = deprecated.pop("boundary_orthogonalization")
+        if deprecated:
+            raise TypeError(f"unexpected keyword arguments {sorted(deprecated)}")
+        super().__init__()
+        self.wavelet = as_wavelet(wavelet)
+        self.mode = mode
+        self.orthogonalization = orthogonalization
+        self.separable = separable
+        self.matrix_wavedec3_dict: dict[tuple[int, ...], MatrixWavedec3] = {}
+        self.matrix_waverec3_dict: dict[tuple[int, ...], MatrixWaverec3] = {}
+        self.axes = tuple(ensure_axes(axes, 3))
+        if self.orthogonalization not in _ORTH_METHODS:
+            raise NotImplementedError
+        self.maxlevel: Optional[int] = None
+        if data is not None:
+            self.transform(data, maxlevel)
+        else:
+            self.data = {}
+
+    def _check_access(self, key: str) -> None:
+        super()._check_access(key)
+        # every level's letters, not only the last level's: a bad key fails before any node is expanded
+        if key not in self and not set(key) <= self._key_chars:
+            raise self._invalid_key(key)
+
+    def _sizes(self, t: torch.Tensor) -> tuple[int, int, int]:
+        return t.shape[self.axes[0]], t.shape[self.axes[1]], t.shape[self.axes[2]]
+
+    def transform(self, data: torch.Tensor, maxlevel: Optional[int] = None) -> "WaveletPacket3D":
+        self.data = {"": data}
+        if maxlevel is None:
+            maxlevel = dwt_max_level(min(self._sizes(data)), self.wavelet.dec_len)
+        self.maxlevel = maxlevel
+        return self
+
+    def _wavedec(self, stacked: torch.Tensor, axes: tuple[int, ...]) -> dict[str, torch.Tensor]:
+        """The eight subbands of a stack of nodes, keyed like the children."""
+        if self.mode == "boundary":
+            shape = tuple(stacked.shape[a] for a in axes)
+            if shape not in self.matrix_wavedec3_dict:
+                self.matrix_wavedec3_dict[shape] = MatrixWavedec3(self.wavelet, level=1, axes=axes,
+                                                                  orthogonalization=self.orthogonalization)
+            a, det = self.matrix_wavedec3_dict[shape](stacked)
+        elif self.separable:
+            a, det = fswavedec3(stacked, self.wavelet, level=1, mode=self.mode, axes=axes)
+        else:
+            a, det = wavedec3(stacked, self.wavelet, level=1, mode=self.mode, axes=axes)
+        return {"aaa": a, **det}
+
+    def _waverec(self, bands: dict[str, torch.Tensor], axes: tuple[int, ...]) -> torch.Tensor:
+        coeffs = (bands["aaa"], {k: bands[k] for k in SUBBANDS_3D[1:]})
+        if self.mode == "boundary":
+            shape = tuple(bands["aaa"].shape[a] for a in axes)
+            if shape not in self.matrix_waverec3_dict:
+                self.matrix_waverec3_dict[shape] = MatrixWaverec3(self.wavelet, axes=axes,
+                                                                  orthogonalization=self.orthogonalization)
+            return self.matrix_waverec3_dict[shape](coeffs)
+        if self.separable:
+            return fswaverec3(coeffs, self.wavelet, axes=axes)
+        return waverec3(coeffs, self.wavelet, axes=axes)
+
+    def _expand_nodes(self, paths: Sequence[str]) -> None:
+        axes = _neg_axes(self.axes, self.data[paths[0]].dim())
+        bands = self._wavedec(self._stack(paths), axes)
+        for i, p in enumerate(paths):
+            for c in SUBBANDS_3D:
+                self.data[p + c] = bands[c][i]
+
+    def reconstruct(self) -> "WaveletPacket3D":
+        """Reconstruct the input from the leaves, one synthesis call per tree level."""
+        if self.maxlevel is None:
+            self.maxlevel = dwt_max_level(min(self._sizes(self[""])), self.wavelet.dec_len)
+        for level in reversed(range(self.maxlevel)):
+            nodes = self.get_natural_order(level)
+            for node in nodes:
+                for child in SUBBANDS_3D:
+                    if node + child not in self:
+                        raise KeyError(f"Key {node + child} not found")
+            axes = _neg_axes(self.axes, self.data[nodes[0] + "aaa"].dim())
+            # all children of the level in one stack [8, nodes, ...]: the seven detail bands reach the synthesis
+            # kernel as equally strided slices of one buffer, without a second copy
+            kids = torch.stack([self.data[n + c] for c in SUBBANDS_3D for n in nodes], 0)
+            kids = kids.reshape((len(SUBBANDS_3D), len(nodes)) + kids.shape[1:])
+            rec = self._waverec(dict(zip(SUBBANDS_3D, kids.unbind(0))), axes)
+            for i, node in enumerate(nodes):
+                r = rec[i]
+                if level > 0:
+                    for ax in axes:
+                        want = self[node].shape[ax]
+                        if r.shape[ax] != want:
+                            assert r.shape[ax] == want + 1, "padding error, please open an issue on GitHub"
+                            r = r.narrow(ax, 0, want)
+                self[node] = r
+        return self
+
+    @staticmethod
+    def get_level(level: int, order: str = "freq"):
+        if order == "freq":
+            return WaveletPacket3D.get_freq_order(level)
+        if order == "natural":
+            return WaveletPacket3D.get_natural_order(level)
+        raise ValueError(f"Unsupported order '{order}'. Choose from 'freq' and 'natural'.")
+
+    @staticmethod
+    def get_natural_order(level: int) -> list[str]:
+        return ["".join(p) for p in product(SUBBANDS_3D, repeat=level)]
+
+    @staticmethod
+    def get_freq_order(level: int) -> list[list[list[str]]]:
+        """3-D frequency order ``[depth][row][col]``: the node grid indexed by the 1-D filter path along each of the
+        three axes, every axis in Gray-code order of its paths (the 3-D form of ``WaveletPacket2D.get_freq_order``)."""
+        to_lh = {"a": "l", "d": "h"}
+        grid: dict[tuple[str, str, str], str] = {}
+        for node in WaveletPacket3D.get_natural_order(level):
+            grid[tuple("".join(to_lh[c] for c in node[a::3]) for a in range(3))] = node
+        order = _graycode_order(level, x="l", y="h")
+        return [[[grid[d, r, c] for c in order] for r in order] for d in order]
