@@ -263,6 +263,31 @@ int wt_swt_inv(int dtype, int levels, int filt_len, const double* g_lo, const do
                int64_t details_band_stride, int64_t batch, int64_t n, void* y, int64_t y_batch_stride,
                const void* const* tables, void* workspace, size_t workspace_bytes, void* stream);
 
+/* 2-D stationary transform (swt2 / iswt2; the reference has no such function, PyWavelets' swt2 with trim_approx=True,
+ * norm=False), built from one level of ONE axis per call.  A pass filters `batch` contiguous rows of n samples with
+ * the periodic forms above at dilation `dilation` (in samples) instead of 2^(j-1):
+ *   along the contiguous axis of [.., H, W] planes: rows of n = W samples (batch = planes * H), dilation d = 2^(j-1);
+ *   along the other axis: each dense H x W plane (row pitch W) is ONE row of n = H W samples at dilation d W, which
+ *   wraps d rows modulo H and keeps the column.
+ * `sets` (1 or 2) band sets run in one call; each array holds one pointer / batch stride per set.
+ *   wt_swt_pass_fwd: x[s] -> lo[s] (f_lo), hi[s] (f_hi)          wt_swt_pass_inv: y[s] = synthesis of lo[s], hi[s]
+ * The two sets take one launch when the pass runs on tiles, one launch each otherwise.  A pass needs no workspace.
+ * wt_swt2_workspace_bytes: the buffers the caller's level cascade keeps between passes for `levels` levels of `batch`
+ * H x W planes, each dense: the two bands of the contiguous-axis pass, plus one approximation plane when levels > 1.
+ * Arguments outside the transform's domain give 0.
+ * wt_swt_pass_plan: how a pass of rows of n samples at `dilation` runs, without running it.  Returns 1 for tiles and
+ * fills tile[4] = {D, M, C, R}: the row seen as M rows of D samples, C rows owned per tile (C == M: whole columns, no
+ * halo), R columns per tile; returns 0 for the per-level kernel (straight from global memory), or a WT_E* code. */
+int wt_swt_pass_plan(int dtype, int inverse, int filt_len, int64_t n, int64_t dilation, int64_t* tile);
+size_t wt_swt2_workspace_bytes(int dtype, int levels, int64_t batch, int64_t h, int64_t w);
+int wt_swt_pass_fwd(int dtype, int filt_len, const double* f_lo, const double* f_hi, int64_t dilation, int sets,
+                    const void* const* x, const int64_t* x_batch_stride, void* const* lo, const int64_t* lo_batch_stride,
+                    void* const* hi, const int64_t* hi_batch_stride, int64_t batch, int64_t n, void* stream);
+int wt_swt_pass_inv(int dtype, int filt_len, const double* g_lo, const double* g_hi, int64_t dilation, int sets,
+                    const void* const* lo, const int64_t* lo_batch_stride, const void* const* hi,
+                    const int64_t* hi_batch_stride, void* const* y, const int64_t* y_batch_stride, int64_t batch,
+                    int64_t n, void* stream);
+
 /* Continuous wavelet transform (ptwt.cwt), src/ptwt/continuous_transform.py:103-137 (per scale: FFT of the
  * filter and the data, product, inverse FFT, diff, crop; then stack), as uniformly partitioned overlap-save in
  * float64 (csrc/cwt.cuh).  Hop H = 2^(fft_log2 - 1), FFT size F = 2H, fft_log2 in 6..12; nb = ceil(n / H).

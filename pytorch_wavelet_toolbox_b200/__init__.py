@@ -26,7 +26,7 @@ from .matrix_fwt import MatrixWavedec, MatrixWaverec, construct_boundary_a, cons
 from .matrix_fwt_nd import MatrixWavedec2, MatrixWavedec3, MatrixWaverec2, MatrixWaverec3
 from .separable import fswavedec2, fswavedec3, fswaverec2, fswaverec3
 from .packets import WaveletPacket, WaveletPacket2D, WaveletPacket3D
-from .stationary import iswt, swt
+from .stationary import iswt, iswt2, swt, swt2
 from .continuous import cwt
 
 __version__ = "0.1.0"
@@ -44,7 +44,7 @@ NEXT_ROW_NAMES = (
 )
 
 #: additions beyond the ptwt API: ptwt has no such names, so install() has nothing to rebind for them
-BEYOND_PTWT_NAMES = ("WaveletPacket3D",)
+BEYOND_PTWT_NAMES = ("WaveletPacket3D", "swt2", "iswt2")
 
 __all__ = list(HOT_PATH_NAMES) + list(NEXT_ROW_NAMES) + list(BEYOND_PTWT_NAMES) + [
     "Wavelet", "WaveletTensorTuple", "WaveletDetailTuple2d", "WaveletDetailDict", "WaveletCoeff1d",

@@ -70,6 +70,12 @@ SIGNATURES = {
                              C.POINTER(_vp), _vp, C.c_size_t, _vp]),
     "wt_swt_inv": (C.c_int, [C.c_int, C.c_int, C.c_int, _f64p, _f64p, _vp, _i64, _vp, _i64, _i64, _i64, _i64, _vp,
                              _i64, C.POINTER(_vp), _vp, C.c_size_t, _vp]),
+    "wt_swt_pass_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, _i64, _i64, _i64p]),
+    "wt_swt2_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64, _i64, _i64]),
+    "wt_swt_pass_fwd": (C.c_int, [C.c_int, C.c_int, _f64p, _f64p, _i64, C.c_int, C.POINTER(_vp), _i64p,
+                                  C.POINTER(_vp), _i64p, C.POINTER(_vp), _i64p, _i64, _i64, _vp]),
+    "wt_swt_pass_inv": (C.c_int, [C.c_int, C.c_int, _f64p, _f64p, _i64, C.c_int, C.POINTER(_vp), _i64p,
+                                  C.POINTER(_vp), _i64p, C.POINTER(_vp), _i64p, _i64, _i64, _vp]),
     "wt_cwt_workspace_bytes": (C.c_size_t, [C.c_int, _i64, _i64, _i64, C.c_int]),
     "wt_cwt_filter_spectra": (C.c_int, [C.c_int, _i64, _vp, _vp, _vp, _vp]),
     "wt_cwt_fwd": (C.c_int, [C.c_int, C.c_int, _i64, _vp, _vp, _vp, C.c_int, _vp, _i64, _i64, _i64, _vp, _i64, _i64,

@@ -22,7 +22,16 @@
 // With D = R the tile is a contiguous chunk of the signal.  Levels whose pad the reference wraps in several
 // non-periodic rounds (_circular_pad with a pad longer than n) run one per launch through a host-built table of
 // source indices (swt_level_*_kernel), as do levels whose halo would not fit a tile.
+//
+// 2-D (swt2, one axis of one level per launch).  The pass along the contiguous axis is the 1-D case on rows of W
+// samples.  The pass along the other axis treats each dense H x W plane as ONE periodic signal of n = H W samples at
+// dilation b = d W: a shift by d W modulo H W moves d rows modulo H and keeps the column, so the signal seen as rows
+// of D = gcd(n, b) = W gcd(H, d) samples splits into independent periodic columns exactly as above.  D need not be a
+// power of two then; a tile's R columns are a power of two that divides it.  That pass filters the two bands of the
+// contiguous-axis pass (lo_W, hi_W) in one launch: items [batch, 2 batch) of the launch are the second band set.
 #pragma once
+
+#include <numeric>
 
 #include "common.cuh"
 
@@ -45,6 +54,12 @@ struct SwtTileParams {
     T* det[SWT_MAXK];          // detail of group level k (k = 0 finest), batch stride det_bs
     int64_t det_bs;
     int64_t batch;
+    // second band set (sets == 2, K == 1 only): items [batch, 2 batch) read a2 and write out2 / det2
+    const T* a2;
+    T* out2;
+    T* det2;
+    int64_t a2_bs, out2_bs, det2_bs;
+    int sets;
     int64_t D, M;              // the signal as M rows of D samples
     int64_t d0;                // dilation of level k = 0 in rows; level k has d0 << k
     int64_t C;                 // rows a CTA owns; C == M: whole columns, no halo
@@ -115,10 +130,12 @@ __global__ void __launch_bounds__(SWT_THREADS, 1) swt_fwd_kernel(const __grid_co
     const int hl = L / 2 - 1;
     const SwtTile t = swt_tile(p, hl, L / 2);
     const int cnt = t.rows << p.lgR;
-    for (int64_t b = blockIdx.y; b < p.batch; b += gridDim.y) {
+    for (int64_t bb = blockIdx.y; bb < p.batch * p.sets; bb += gridDim.y) {
+        const bool s2 = bb >= p.batch;
+        const int64_t b = s2 ? bb - p.batch : bb;
         T* A = reinterpret_cast<T*>(smem_raw);
         T* B = A + cnt;
-        swt_stage(A, p.a + b * p.a_bs, p, t, 0, t.rows);
+        swt_stage(A, s2 ? p.a2 + b * p.a2_bs : p.a + b * p.a_bs, p, t, 0, t.rows);
         __syncthreads();
         int lo = 0, hi = t.rows;
         for (int k = 0; k < p.K; ++k) {
@@ -126,8 +143,8 @@ __global__ void __launch_bounds__(SWT_THREADS, 1) swt_fwd_kernel(const __grid_co
             const int olo = t.full ? 0 : lo + (int)(dk * hl);
             const int ohi = t.full ? hi : hi - (int)(dk * (L / 2));
             const bool last = k == p.K - 1;
-            T* det = p.det[k] + b * p.det_bs;
-            T* out = p.out + b * p.out_bs;
+            T* det = s2 ? p.det2 + b * p.det2_bs : p.det[k] + b * p.det_bs;
+            T* out = s2 ? p.out2 + b * p.out2_bs : p.out + b * p.out_bs;
             auto emit = [&](int row, int col, T vlo, T vhi) {
                 if (!last) B[(row << p.lgR) + col] = vlo;
                 if (row >= t.HLr && row < t.own_hi) {
@@ -192,20 +209,22 @@ __global__ void __launch_bounds__(SWT_THREADS, 1) swt_inv_kernel(const __grid_co
     const int hl = L / 2 - 1;
     const SwtTile t = swt_tile(p, L / 2, hl);
     const int cnt = t.rows << p.lgR;
-    for (int64_t b = blockIdx.y; b < p.batch; b += gridDim.y) {
+    for (int64_t bb = blockIdx.y; bb < p.batch * p.sets; bb += gridDim.y) {
+        const bool s2 = bb >= p.batch;
+        const int64_t b = s2 ? bb - p.batch : bb;
         T* A = reinterpret_cast<T*>(smem_raw);
         T* B = A + cnt;
         T* Dt = B + cnt;
-        swt_stage(A, p.a + b * p.a_bs, p, t, 0, t.rows);
+        swt_stage(A, s2 ? p.a2 + b * p.a2_bs : p.a + b * p.a_bs, p, t, 0, t.rows);
         int lo = 0, hi = t.rows;
         for (int k = p.K - 1; k >= 0; --k) {
             const int64_t dk = p.d0 << k;
-            swt_stage(Dt, p.det[k] + b * p.det_bs, p, t, lo, hi);
+            swt_stage(Dt, s2 ? p.det2 + b * p.det2_bs : p.det[k] + b * p.det_bs, p, t, lo, hi);
             __syncthreads();
             const int olo = t.full ? 0 : lo + (int)(dk * (L / 2));
             const int ohi = t.full ? hi : hi - (int)(dk * hl);
             const bool last = k == 0;
-            T* out = p.out + b * p.out_bs;
+            T* out = s2 ? p.out2 + b * p.out2_bs : p.out + b * p.out_bs;
             auto emit = [&](int row, int col, T v) {
                 if (!last) B[(row << p.lgR) + col] = v;
                 else if (row >= t.HLr && row < t.own_hi) out[(t.i0 + row - t.HLr) * p.D + t.c0 + col] = v;
@@ -326,11 +345,13 @@ static inline int swt_log2(int64_t v) {
     return l;
 }
 
-// Levels 1..levels, finest first.  A level with a table always runs alone.  Otherwise the group starting at level
-// j sees the signal as rows of D = gcd(n, 2^(j-1)) samples; it takes whole columns when a tile of at least one
-// 32-byte sector per row holds all M = n / D rows, else a halo tile of as many levels as keep the halo within a
-// quarter of the tile.
-static int swt_plan(int es, bool inverse, int levels, int L, int64_t n, const void* const* tables, SwtStep* steps) {
+// Levels 1..levels, finest first; level j has dilation b0 2^(j-1) (1-D: b0 = 1; the 2-D pass along the slow axis:
+// b0 = d W).  A level with a table always runs alone.  Otherwise the group starting at level j sees the signal as rows
+// of D = gcd(n, b0 2^(j-1)) samples; it takes whole columns when a tile of at least one 32-byte sector per row holds
+// all M = n / D rows, else a halo tile of as many levels as keep the halo within a quarter of the tile.  A tile's
+// column count R is a power of two that divides D (for b0 = 1, D is a power of two itself).
+static int swt_plan(int es, bool inverse, int levels, int L, int64_t n, const void* const* tables, SwtStep* steps,
+                    int64_t b0 = 1) {
     const int64_t cap = (inverse ? SWT_INV_BUF_BYTES : SWT_FWD_BUF_BYTES) / es;
     int ns = 0;
     for (int j = 1; j <= levels;) {
@@ -342,19 +363,20 @@ static int swt_plan(int es, bool inverse, int levels, int L, int64_t n, const vo
             ++j;
             continue;
         }
-        const int64_t d = int64_t(1) << (j - 1);
-        const int64_t D = std::min(d, n & -n);
+        const int64_t d = b0 << (j - 1);
+        const int64_t D = std::gcd(n, d);
+        const int64_t Dp = D & -D;             // largest power of two dividing D
         const int64_t M = n / D;
         int kmax = 0;
         while (j + kmax <= levels && kmax < SWT_MAXK && !(tables && tables[j + kmax - 1])) ++kmax;
-        const int64_t rmin = std::min<int64_t>(D, 32 / es);
+        const int64_t rmin = std::min<int64_t>(Dp, 32 / es);
         s.D = D;
         s.d0 = d / D;
         if (M * rmin <= cap) {
             s.tiled = true;
             s.K = kmax;
             s.C = M;
-            s.lgR = swt_log2(std::min<int64_t>(D, cap / M));
+            s.lgR = swt_log2(std::min<int64_t>(Dp, cap / M));
         } else {
             const int64_t rows_cap = cap / rmin;
             int K = 0;
@@ -376,7 +398,7 @@ static int swt_plan(int es, bool inverse, int levels, int L, int64_t n, const vo
 template <typename T, int LT>
 static cudaError_t swt_launch_tile(bool inverse, const SwtTileParams<T>& p, size_t smem, cudaStream_t st) {
     const int64_t ntile = (p.M + p.C - 1) / p.C;
-    dim3 grid((unsigned)(ntile * (p.D / p.R)), (unsigned)std::min<int64_t>(p.batch, 65535));
+    dim3 grid((unsigned)(ntile * (p.D / p.R)), (unsigned)std::min<int64_t>(p.batch * p.sets, 65535));
     const size_t most = (inverse ? 3 * SWT_INV_BUF_BYTES : 2 * SWT_FWD_BUF_BYTES) + 64;
     cudaError_t e;
     if (inverse) {

@@ -872,7 +872,7 @@ static int swt_fwd_t(int levels, int L, const double* f_lo, const double* f_hi, 
             memset(&p, 0, sizeof(p));
             p.a = in; p.a_bs = in_bs; p.out = a_out; p.out_bs = a_bs;
             for (int k = 0; k < S.K; ++k) p.det[k] = out + (int64_t)(levels + 1 - (S.j0 + k)) * band;
-            p.det_bs = obs; p.batch = batch;
+            p.det_bs = obs; p.batch = batch; p.sets = 1;
             p.D = S.D; p.M = n / S.D; p.d0 = S.d0; p.C = S.C;
             p.K = S.K; p.R = S.R; p.lgR = S.lgR; p.L = L;
             for (int m = 0; m < L; ++m) { p.f0[m] = (T)f_lo[m]; p.f1[m] = (T)f_hi[m]; }
@@ -916,7 +916,7 @@ static int swt_inv_t(int levels, int L, const double* g_lo, const double* g_hi, 
             memset(&p, 0, sizeof(p));
             p.a = in; p.a_bs = in_bs; p.out = a_out; p.out_bs = a_bs;
             for (int k = 0; k < S.K; ++k) p.det[k] = const_cast<T*>(det) + (int64_t)(levels - (S.j0 + k)) * band;
-            p.det_bs = dbs; p.batch = batch;
+            p.det_bs = dbs; p.batch = batch; p.sets = 1;
             p.D = S.D; p.M = n / S.D; p.d0 = S.d0; p.C = S.C;
             p.K = S.K; p.R = S.R; p.lgR = S.lgR; p.L = L;
             for (int m = 0; m < L; ++m) { p.f0[m] = (T)g_lo[m]; p.f1[m] = (T)g_hi[m]; }
@@ -937,6 +937,67 @@ static int swt_inv_t(int levels, int L, const double* g_lo, const double* g_hi, 
         in = a_out;
         in_bs = a_bs;
     }
+    return 0;
+}
+
+// One level of one axis of the 2-D transform: the first group of swt_plan(levels = 1) at dilation b, on `sets` (1 or
+// 2) band sets.  A tile takes both sets in one launch; the per-level kernel runs one launch per set.  Analysis: in0
+// is the input, out0 / out1 the low / high band.  Synthesis: in0 / in1 the low / high band, out0 the result.
+template <typename T>
+static int swt_pass_t(bool inverse, int L, const double* f0, const double* f1, int64_t b, int sets,
+                      const void* const* in0, const int64_t* in0_bs, const void* const* in1, const int64_t* in1_bs,
+                      void* const* out0, const int64_t* out0_bs, void* const* out1, const int64_t* out1_bs,
+                      int64_t batch, int64_t n, cudaStream_t st) {
+    SwtStep steps[64];
+    swt_plan(sizeof(T), inverse, 1, L, n, nullptr, steps, b);
+    const SwtStep& S = steps[0];
+    cudaError_t e = cudaSuccess;
+    if (S.tiled) {
+        SwtTileParams<T> p;
+        memset(&p, 0, sizeof(p));
+        p.a = (const T*)in0[0]; p.a_bs = in0_bs[0];
+        p.out = (T*)out0[0]; p.out_bs = out0_bs[0];
+        p.det[0] = inverse ? (T*)in1[0] : (T*)out1[0];
+        p.det_bs = inverse ? in1_bs[0] : out1_bs[0];
+        if (sets == 2) {
+            p.a2 = (const T*)in0[1]; p.a2_bs = in0_bs[1];
+            p.out2 = (T*)out0[1]; p.out2_bs = out0_bs[1];
+            p.det2 = inverse ? (T*)in1[1] : (T*)out1[1];
+            p.det2_bs = inverse ? in1_bs[1] : out1_bs[1];
+        }
+        p.batch = batch; p.sets = sets;
+        p.D = S.D; p.M = n / S.D; p.d0 = S.d0; p.C = S.C;
+        p.K = 1; p.R = S.R; p.lgR = S.lgR; p.L = L;
+        for (int m = 0; m < L; ++m) { p.f0[m] = (T)f0[m]; p.f1[m] = (T)f1[m]; }
+        e = swt_run_tile<T>(inverse, p, st);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if (e != cudaSuccess) return cuda_fail(e, inverse ? "swt_inv_kernel" : "swt_fwd_kernel");
+        return 0;
+    }
+    for (int s = 0; s < sets; ++s) {
+        SwtLevelParams<T> p;
+        memset(&p, 0, sizeof(p));
+        p.a0 = (const T*)in0[s]; p.a0_bs = in0_bs[s];
+        if (inverse) { p.a1 = (const T*)in1[s]; p.a1_bs = in1_bs[s]; }
+        p.o0 = (T*)out0[s]; p.o0_bs = out0_bs[s];
+        if (!inverse) { p.o1 = (T*)out1[s]; p.o1_bs = out1_bs[s]; }
+        p.batch = batch; p.n = n; p.d = b; p.L = L;
+        for (int m = 0; m < L; ++m) { p.f0[m] = (T)f0[m]; p.f1[m] = (T)f1[m]; }
+        e = swt_run_level<T>(inverse, p, st);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if (e != cudaSuccess) return cuda_fail(e, "swt_level_kernel");
+    }
+    return 0;
+}
+
+static const double g_unit_tap = 1.0;   // a non-NULL tap array for wt_swt_pass_plan's argument check
+
+static int swt_pass_check(int dtype, int filt_len, const double* t0, const double* t1, int64_t dilation, int sets,
+                          int64_t batch, int64_t n) {
+    int rc = swt_check(dtype, 1, filt_len, t0, t1, batch, n);
+    if (rc) return rc;
+    if (dilation < 1) return fail(WT_EINVAL, "dilation %lld", (long long)dilation);
+    if (sets != 1 && sets != 2) return fail(WT_EINVAL, "sets %d (1 or 2)", sets);
     return 0;
 }
 
@@ -1135,6 +1196,58 @@ int wt_swt_inv(int dtype, int levels, int filt_len, const double* g_lo, const do
     return swt_inv_t<double>(levels, filt_len, g_lo, g_hi, (const double*)approx, approx_batch_stride,
                              (const double*)details, details_batch_stride, details_band_stride, batch, n, (double*)y,
                              y_batch_stride, tables, (double*)workspace, workspace_bytes, st);
+}
+
+int wt_swt_pass_plan(int dtype, int inverse, int filt_len, int64_t n, int64_t dilation, int64_t* tile) {
+    int rc = swt_pass_check(dtype, filt_len, &g_unit_tap, &g_unit_tap, dilation, 1, 0, n);
+    if (rc) return rc;
+    if (!tile) return fail(WT_EINVAL, "NULL argument");
+    SwtStep steps[64];
+    swt_plan(dtype == WT_F64 ? 8 : 4, inverse != 0, 1, filt_len, n, nullptr, steps, dilation);
+    const SwtStep& S = steps[0];
+    tile[0] = S.D; tile[1] = S.tiled ? n / S.D : 0; tile[2] = S.C; tile[3] = S.R;
+    return S.tiled ? 1 : 0;
+}
+
+size_t wt_swt2_workspace_bytes(int dtype, int levels, int64_t batch, int64_t h, int64_t w) {
+    if ((dtype != WT_F32 && dtype != WT_F64) || levels < 1 || levels > 40 || batch < 1 || h < 1 || w < 1) return 0;
+    const size_t plane = (size_t)(batch * h * w) * (dtype == WT_F64 ? 8 : 4);
+    return plane * (levels > 1 ? 3 : 2);
+}
+
+int wt_swt_pass_fwd(int dtype, int filt_len, const double* f_lo, const double* f_hi, int64_t dilation, int sets,
+                    const void* const* x, const int64_t* x_batch_stride, void* const* lo, const int64_t* lo_batch_stride,
+                    void* const* hi, const int64_t* hi_batch_stride, int64_t batch, int64_t n, void* stream) {
+    int rc = swt_pass_check(dtype, filt_len, f_lo, f_hi, dilation, sets, batch, n);
+    if (rc) return rc;
+    if (batch == 0) return 0;
+    if (!x || !x_batch_stride || !lo || !lo_batch_stride || !hi || !hi_batch_stride) return fail(WT_EINVAL, "NULL argument");
+    for (int s = 0; s < sets; ++s)
+        if (!x[s] || !lo[s] || !hi[s]) return fail(WT_EINVAL, "NULL band of set %d", s);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32)
+        return swt_pass_t<float>(false, filt_len, f_lo, f_hi, dilation, sets, x, x_batch_stride, nullptr, nullptr, lo,
+                                 lo_batch_stride, hi, hi_batch_stride, batch, n, st);
+    return swt_pass_t<double>(false, filt_len, f_lo, f_hi, dilation, sets, x, x_batch_stride, nullptr, nullptr, lo,
+                              lo_batch_stride, hi, hi_batch_stride, batch, n, st);
+}
+
+int wt_swt_pass_inv(int dtype, int filt_len, const double* g_lo, const double* g_hi, int64_t dilation, int sets,
+                    const void* const* lo, const int64_t* lo_batch_stride, const void* const* hi,
+                    const int64_t* hi_batch_stride, void* const* y, const int64_t* y_batch_stride, int64_t batch,
+                    int64_t n, void* stream) {
+    int rc = swt_pass_check(dtype, filt_len, g_lo, g_hi, dilation, sets, batch, n);
+    if (rc) return rc;
+    if (batch == 0) return 0;
+    if (!lo || !lo_batch_stride || !hi || !hi_batch_stride || !y || !y_batch_stride) return fail(WT_EINVAL, "NULL argument");
+    for (int s = 0; s < sets; ++s)
+        if (!lo[s] || !hi[s] || !y[s]) return fail(WT_EINVAL, "NULL band of set %d", s);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == WT_F32)
+        return swt_pass_t<float>(true, filt_len, g_lo, g_hi, dilation, sets, lo, lo_batch_stride, hi, hi_batch_stride,
+                                 y, y_batch_stride, nullptr, nullptr, batch, n, st);
+    return swt_pass_t<double>(true, filt_len, g_lo, g_hi, dilation, sets, lo, lo_batch_stride, hi, hi_batch_stride, y,
+                              y_batch_stride, nullptr, nullptr, batch, n, st);
 }
 
 const char* wt_last_error(void) { return g_err; }

@@ -13,6 +13,12 @@ kernels read it from a table (only short signals with an explicit ``level`` get 
 
 Outputs are views of one packed ``[batch, level + 1, pitch]`` buffer (rows 16-byte aligned); ``iswt`` consumes such
 views without a copy.  CPU tensors are staged to the current CUDA device and back, as in :func:`wavedec`.
+
+``swt2`` / ``iswt2`` are the 2-D transform (PyWavelets' ``swt2`` with ``trim_approx=True``, ``norm=False``; the
+reference has none).  Each level is two one-axis passes on the same kernels (``wt_swt_pass_fwd`` / ``wt_swt_pass_inv``):
+rows of W samples along ``axes[1]``, then each H x W plane as one periodic signal of H W samples at dilation d W along
+``axes[0]``.  The extension is exactly periodic at every level, including dilations longer than the extent: there is
+no reference ``swt2`` whose multi-round padding could be copied.
 """
 from __future__ import annotations
 
@@ -25,11 +31,13 @@ import torch
 import torch.nn.functional as F
 
 from . import _native as N
-from ._shape import AxisHint, check_dtype, check_tensor, fold, round_up, unfold
+from ._shape import AxisHint, check_dtype, check_tensor, ensure_axes, fold, round_up, unfold
 from ._wavelets import any_requires_grad, as_wavelet, filter_bank, swt_max_level, taps_in_dtype
-from .fwt import ROW_ALIGN_BYTES, _compute_device, _dtype_code, _pack_bands, _same_device_dtype, pinned_empty
+from .constants import WaveletDetailTuple2d
+from .fwt import (BAND_ALIGN_BYTES, ROW_ALIGN_BYTES, _compute_device, _dtype_code, _fold_coeff_tensors, _pack_bands,
+                  _same_device_dtype, pinned_empty)
 
-__all__ = ["swt", "iswt"]
+__all__ = ["swt", "iswt", "swt2", "iswt2"]
 
 
 # --------------------------------------------------------------------------------------
@@ -259,22 +267,22 @@ class _IswtAdjointFunction(torch.autograd.Function):
         return _IswtFunction.apply(ctx.fb, ctx.L, *[u.contiguous() for u in us]), None, None, None
 
 
-def _check_taps_without_grad(wav: Any) -> None:
+def _check_taps_without_grad(wav: Any, what: str = "swt/iswt") -> None:
     if torch.is_grad_enabled() and any_requires_grad(wav):
         raise NotImplementedError(
-            "swt/iswt compute gradients with respect to the data only, not with respect to learnable filter taps; "
+            f"{what} compute gradients with respect to the data only, not with respect to learnable filter taps; "
             "pass plain filters or call under torch.no_grad()."
         )
 
 
-def _filter_bank(wavelet: Any):
+def _filter_bank(wavelet: Any, what: str = "swt/iswt"):
     wav = as_wavelet(wavelet)
     fb = filter_bank(wav)
     L = len(fb[0])
     if any(len(f) != L for f in fb):
         raise ValueError("all four filters of the wavelet must have the same length")
     if L < 2 or L > N.WT_MAX_FILT_LEN or L % 2:
-        raise ValueError(f"swt/iswt need an even filter length in 2..{N.WT_MAX_FILT_LEN}, got {L}")
+        raise ValueError(f"{what} need an even filter length in 2..{N.WT_MAX_FILT_LEN}, got {L}")
     return wav, fb, L
 
 
@@ -357,6 +365,302 @@ def iswt(coeffs: Sequence[torch.Tensor], wavelet: Any, *, axis: AxisHint = None)
             details = [t.to(dev, non_blocking=True) for t in details]
         g_lo, g_hi = _window_taps(fb, approx.dtype, inverse=True)
         y = run_synthesis(approx, details, g_lo, g_hi, L, tables_inverse=True, transpose=False)
+        if on_host:
+            host = pinned_empty(y.shape, y.dtype)
+            host.copy_(y, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            y = host
+    return unfold(y, f)
+
+
+# --------------------------------------------------------------------------------------
+# 2-D: one launch per axis pass, two passes per level
+# --------------------------------------------------------------------------------------
+def _dense_planes(t: torch.Tensor) -> torch.Tensor:
+    """``t [B, H, W]`` itself when every plane is dense with row pitch W (what the pass along axes[0] reads as one
+    signal of H W samples), else a contiguous copy."""
+    _, H, W = t.shape
+    if (W == 1 or t.stride(2) == 1) and (H == 1 or t.stride(1) == W):
+        return t
+    return t.contiguous()
+
+
+def _rows(t: torch.Tensor) -> tuple[torch.Tensor, int]:
+    """``t [B, H, W]`` as B H rows of W samples one stride apart (the pass along axes[1]): (tensor, row stride)."""
+    B, H, W = t.shape
+    if W == 1 or t.stride(2) == 1:
+        if H == 1:
+            return t, t.stride(0)
+        if B == 1 or t.stride(0) == H * t.stride(1):
+            return t, t.stride(1)
+    return t.contiguous(), W
+
+
+def _pack_planes(bands: list[torch.Tensor]) -> tuple[torch.Tensor, int, int]:
+    """(tensor at band 0, band stride, batch stride) of equally shaped ``[B, H, W]`` bands with dense planes: the bands
+    themselves when they are equally strided planes of one buffer (what :func:`swt2` returns), else one gather."""
+    _, H, W = bands[0].shape
+    base, step, st, bs = _pack_bands(bands, 1)
+    if H > 1 and st[0] != W:
+        base = torch.stack(bands, 1)
+        step, bs = base.stride(1), base.stride(0)
+    return base, step, bs
+
+
+def _ptrs(*addrs: int):
+    return (C.c_void_p * len(addrs))(*addrs)
+
+
+def _i64s(*vals: int):
+    return (C.c_int64 * len(vals))(*vals)
+
+
+def _pass(inverse: bool, code: int, taps, L: int, dilation: int, in0, in0_bs, in1, in1_bs, out0, out0_bs, batch: int,
+          n: int, stream) -> None:
+    """One wt_swt_pass_fwd / wt_swt_pass_inv call; in* / out* are tuples of addresses and batch strides, one per band
+    set.  Analysis: in0 -> out0 (low), in1 (high, an output).  Synthesis: in0 (low), in1 (high) -> out0."""
+    lo_arr, lo_p = N.f64_array(taps[0])
+    hi_arr, hi_p = N.f64_array(taps[1])
+    sets = len(in0)
+    lib = N.load()
+    if inverse:
+        rc = lib.wt_swt_pass_inv(code, L, lo_p, hi_p, dilation, sets, _ptrs(*in0), _i64s(*in0_bs), _ptrs(*in1),
+                                 _i64s(*in1_bs), _ptrs(*out0), _i64s(*out0_bs), batch, n, stream)
+    else:
+        rc = lib.wt_swt_pass_fwd(code, L, lo_p, hi_p, dilation, sets, _ptrs(*in0), _i64s(*in0_bs), _ptrs(*out0),
+                                 _i64s(*out0_bs), _ptrs(*in1), _i64s(*in1_bs), batch, n, stream)
+    N.check(rc, "wt_swt_pass_inv" if inverse else "wt_swt_pass_fwd")
+
+
+def _workspace2(code: int, levels: int, B: int, H: int, W: int, dtype, device) -> tuple[int, int, int]:
+    """Addresses of the workspace planes: the two bands of the pass along axes[1] and the running approximation."""
+    ws_bytes = int(N.load().wt_swt2_workspace_bytes(code, levels, B, H, W))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
+    plane = B * H * W * torch.empty((), dtype=dtype).element_size()
+    base = ws.data_ptr()
+    return ws, base, base + plane, base + 2 * plane
+
+
+def band_pitch(n: int, dtype: torch.dtype) -> int:
+    """Elements between the planes of one item of :func:`swt2`'s packed buffer: H W rounded up to 128 bytes."""
+    es = torch.empty((), dtype=dtype).element_size()
+    return round_up(n, BAND_ALIGN_BYTES // es)
+
+
+def run_analysis2(x: torch.Tensor, f_lo, f_hi, levels: int, L: int) -> torch.Tensor:
+    """``x [B, H, W]`` (CUDA) -> packed ``[B, 3 levels + 1, pitch]``: cA_J, then (cH_j, cV_j, cD_j) for j = J..1, each
+    band a dense H x W plane at the start of its row."""
+    B, H, W = x.shape
+    n = H * W
+    out = torch.empty((B, 3 * levels + 1, band_pitch(n, x.dtype)), dtype=x.dtype, device=x.device)
+    if out.numel() == 0 or n == 0:
+        return out
+    code, es = _dtype_code(x.dtype), x.element_size()
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    x, rs = _rows(x)
+    ws, lo_w, hi_w, a_ws = _workspace2(code, levels, B, H, W, x.dtype, x.device)
+    obs, band = out.stride(0), out.stride(1) * es
+    src, src_rs = x.data_ptr(), rs
+    for j in range(1, levels + 1):
+        d = 1 << (j - 1)
+        _pass(False, code, (f_lo, f_hi), L, d, (src,), (src_rs,), (hi_w,), (W,), (lo_w,), (W,), B * H, W, stream)
+        k = out.data_ptr() + (1 + 3 * (levels - j)) * band        # cH_j; cV_j and cD_j follow
+        a_dst, a_bs = (out.data_ptr(), obs) if j == levels else (a_ws, n)
+        # set 0: lo_W -> (cA_j, cH_j); set 1: hi_W -> (cV_j, cD_j)
+        _pass(False, code, (f_lo, f_hi), L, d * W, (lo_w, hi_w), (n, n), (k, k + 2 * band), (obs, obs),
+              (a_dst, k + band), (a_bs, obs), B, n, stream)
+        src, src_rs = a_ws, W
+    del ws, x
+    return out
+
+
+def run_synthesis2(approx: torch.Tensor, details: Sequence[torch.Tensor], g_lo, g_hi, L: int) -> torch.Tensor:
+    """``approx [B, H, W]`` and ``details`` = [cH_J, cV_J, cD_J, ..., cH_1, cV_1, cD_1] (CUDA) -> ``[B, H, W]``."""
+    levels = len(details) // 3
+    B, H, W = approx.shape
+    n = H * W
+    y = torch.empty((B, H, W), dtype=approx.dtype, device=approx.device)
+    if y.numel() == 0:
+        return y
+    code, es = _dtype_code(approx.dtype), approx.element_size()
+    stream = torch.cuda.current_stream(approx.device).cuda_stream
+    a = _dense_planes(approx)
+    base, step, dbs = _pack_planes(list(details))
+    ws, lo_w, hi_w, a_ws = _workspace2(code, levels, B, H, W, approx.dtype, approx.device)
+    cur, cur_bs = a.data_ptr(), a.stride(0)
+    for j in range(levels, 0, -1):
+        d = 1 << (j - 1)
+        k = base.data_ptr() + 3 * (levels - j) * step * es       # cH_j; cV_j and cD_j follow
+        kv, kd = k + step * es, k + 2 * step * es
+        # set 0: (cA_j, cH_j) -> lo_W; set 1: (cV_j, cD_j) -> hi_W
+        _pass(True, code, (g_lo, g_hi), L, d * W, (cur, kv), (cur_bs, dbs), (k, kd), (dbs, dbs), (lo_w, hi_w),
+              (n, n), B, n, stream)
+        dst = y.data_ptr() if j == 1 else a_ws
+        _pass(True, code, (g_lo, g_hi), L, d, (lo_w,), (W,), (hi_w,), (W,), (dst,), (W,), B * H, W, stream)
+        cur, cur_bs = a_ws, n
+    del ws, a, base
+    return y
+
+
+def _bands2(packed: torch.Tensor, levels: int, H: int, W: int) -> list[torch.Tensor]:
+    """The 3 levels + 1 ``[B, H, W]`` views of a packed buffer."""
+    B = packed.shape[0]
+    return [packed[:, k, :H * W].view(B, H, W) for k in range(3 * levels + 1)]
+
+
+def _swt2_adjoint(g: torch.Tensor, fb, levels: int, L: int, H: int, W: int) -> torch.Tensor:
+    """Adjoint of swt2: packed gradient -> ``[B, H, W]`` (the pitch padding is not read)."""
+    f_lo, f_hi = _window_taps(fb, g.dtype, inverse=False)
+    bands = _bands2(g.contiguous(), levels, H, W)
+    return run_synthesis2(bands[0], bands[1:], f_lo, f_hi, L)
+
+
+def _iswt2_adjoint(gy: torch.Tensor, fb, levels: int, L: int) -> tuple:
+    """Adjoint of iswt2: ``[B, H, W]`` gradient -> the gradients of approx and the 3 levels details."""
+    f_lo, f_hi = _window_taps(fb, gy.dtype, inverse=True)
+    _, H, W = gy.shape
+    return tuple(_bands2(run_analysis2(gy, f_lo, f_hi, levels, L), levels, H, W))
+
+
+class _Swt2Function(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, fb, levels, L):
+        ctx.fb, ctx.levels, ctx.L, ctx.hw = fb, levels, L, tuple(x.shape[-2:])
+        f_lo, f_hi = _window_taps(fb, x.dtype, inverse=False)
+        return run_analysis2(x, f_lo, f_hi, levels, L)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _Swt2AdjointFunction.apply(g, ctx.fb, ctx.levels, ctx.L, *ctx.hw), None, None, None
+
+
+class _Swt2AdjointFunction(torch.autograd.Function):
+    """The backward pass of swt2 as a differentiable map; its own adjoint is swt2, written into the packed layout
+    with zeros in the pitch padding."""
+
+    @staticmethod
+    def forward(ctx, g, fb, levels, L, H, W):
+        ctx.fb, ctx.levels, ctx.L, ctx.n, ctx.pitch = fb, levels, L, H * W, g.shape[-1]
+        return _swt2_adjoint(g, fb, levels, L, H, W)
+
+    @staticmethod
+    def backward(ctx, u):
+        packed = _Swt2Function.apply(u, ctx.fb, ctx.levels, ctx.L)
+        return F.pad(packed[..., :ctx.n], (0, ctx.pitch - ctx.n)), None, None, None, None, None
+
+
+class _Iswt2Function(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, fb, L, approx, *details):
+        ctx.fb, ctx.L, ctx.levels = fb, L, len(details) // 3
+        g_lo, g_hi = _window_taps(fb, approx.dtype, inverse=True)
+        return run_synthesis2(approx, details, g_lo, g_hi, L)
+
+    @staticmethod
+    def backward(ctx, gy):
+        return (None, None) + _Iswt2AdjointFunction.apply(gy, ctx.fb, ctx.levels, ctx.L)
+
+
+class _Iswt2AdjointFunction(torch.autograd.Function):
+    """The backward pass of iswt2 as a differentiable map; its own adjoint is iswt2."""
+
+    @staticmethod
+    def forward(ctx, gy, fb, levels, L):
+        ctx.fb, ctx.L = fb, L
+        return _iswt2_adjoint(gy, fb, levels, L)
+
+    @staticmethod
+    def backward(ctx, *us):
+        return _Iswt2Function.apply(ctx.fb, ctx.L, *us), None, None, None
+
+
+def swt2(data: torch.Tensor, wavelet: Any, level: Optional[int] = None, *, axes: tuple[int, int] = (-2, -1)):
+    """2-D stationary wavelet transform, ``(cA_J, (cH_J, cV_J, cD_J), ..., (cH_1, cV_1, cD_1))`` with the details as
+    :class:`WaveletDetailTuple2d`, every band shaped like the input: PyWavelets' ``swt2`` with ``trim_approx=True``
+    and ``norm=False``, in the container of :func:`wavedec2`.
+
+    Level j (dilation d = 2^(j-1), hl = L/2 - 1, window taps f = dec[::-1]) computes, with a the filter along
+    ``axes[0]`` and b the one along ``axes[1]``:
+
+        c_ab[r, s] = sum_m sum_k f_a[m] f_b[k] A_{j-1}[(r + d (m - hl)) mod H, (s + d (k - hl)) mod W]
+
+    cA = (lo, lo), cH = (hi, lo), cV = (lo, hi), cD = (hi, hi): the orientation of :func:`wavedec2`'s bands.  The
+    extension is periodic at every level, also where d (L - 1) exceeds an extent (the reference has no ``swt2``, and
+    its 1-D ``swt``'s multi-round padding is not copied here).  The default level is the largest that
+    ``swt_max_level`` allows along both axes; a level <= 0 returns ``(data,)``.
+    """
+    check_tensor(data)
+    check_dtype(data)
+    x, f = fold(data, 2, axes)
+    H, W = int(x.shape[-2]), int(x.shape[-1])
+    if level is None:
+        level = min(swt_max_level(H), swt_max_level(W))
+    if level <= 0:
+        return (unfold(x, f),)
+    wav, fb, L = _filter_bank(wavelet, "swt2/iswt2")
+    _check_taps_without_grad(wav, "swt2/iswt2")
+    dev = _compute_device(x)
+    on_host = not x.is_cuda
+    with torch.cuda.device(dev):
+        if torch.is_grad_enabled() and x.requires_grad:
+            packed = _Swt2Function.apply(x.to(dev), fb, level, L)
+            bands = _bands2(packed, level, H, W)
+            if on_host:
+                bands = [t.cpu() for t in bands]
+        else:
+            xd = x.to(dev, non_blocking=True) if on_host else x
+            f_lo, f_hi = _window_taps(fb, x.dtype, inverse=False)
+            packed = run_analysis2(xd, f_lo, f_hi, level, L)
+            if on_host:
+                host = pinned_empty(packed.shape, packed.dtype)
+                host.copy_(packed, non_blocking=True)
+                torch.cuda.current_stream(dev).synchronize()
+                packed = host
+            bands = _bands2(packed, level, H, W)
+    out: list[Any] = [unfold(bands[0], f)]
+    for k in range(level):
+        h, v, d = bands[1 + 3 * k: 4 + 3 * k]
+        out.append(WaveletDetailTuple2d(unfold(h, f), unfold(v, f), unfold(d, f)))
+    return tuple(out)
+
+
+def iswt2(coeffs, wavelet: Any, *, axes: AxisHint = None) -> torch.Tensor:
+    """Inverse of :func:`swt2`: per level and axis the synthesis of include/wtb200.h with g = 0.5 rec, i.e. the mean
+    of the four branches.  Reads :func:`swt2`'s own views without a copy; other layouts are gathered once."""
+    lead = check_tensor(coeffs[0])
+    check_dtype(lead)
+    ensure_axes(axes, 2)
+    for el in coeffs[1:]:
+        if not isinstance(el, tuple) or len(el) != 3:
+            raise ValueError(
+                f"Unexpected detail coefficient type: {type(el)}. Detail coefficients must be a 3-tuple of "
+                "tensors as returned by swt2."
+            )
+    flat: list[torch.Tensor] = [lead]
+    for el in coeffs[1:]:
+        flat.extend(el)
+    folded, f = _fold_coeff_tensors(flat, 2, axes)
+    _same_device_dtype(folded)
+    approx, details = folded[0], folded[1:]
+    if not details:
+        return unfold(approx, f)
+    for t in details:
+        if t.shape != approx.shape:
+            raise RuntimeError(f"all swt2 bands must have the same shape, got {list(approx.shape)} for the "
+                               f"approximation and {list(t.shape)} for a detail")
+    wav, fb, L = _filter_bank(wavelet, "swt2/iswt2")
+    _check_taps_without_grad(wav, "swt2/iswt2")
+    dev = _compute_device(approx)
+    on_host = not approx.is_cuda
+    with torch.cuda.device(dev):
+        if torch.is_grad_enabled() and any(t.requires_grad for t in folded):
+            y = _Iswt2Function.apply(fb, L, *[t.to(dev) for t in folded])
+            return unfold(y.cpu() if on_host else y, f)
+        if on_host:
+            approx = approx.to(dev, non_blocking=True)
+            details = [t.to(dev, non_blocking=True) for t in details]
+        g_lo, g_hi = _window_taps(fb, approx.dtype, inverse=True)
+        y = run_synthesis2(approx, details, g_lo, g_hi, L)
         if on_host:
             host = pinned_empty(y.shape, y.dtype)
             host.copy_(y, non_blocking=True)
